@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- training images/sec of the Council-GAN step (dis_update + dis_council_update + gen_update).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One "step" = one full training iteration (train.py:241-250 order) over one synthetic minibatch.
@@ -12,12 +12,14 @@ Prints ONE JSON line (rank 0).  `value` = images/sec with inputs resident in HBM
 the public Council_Trainer API with HOST (pinned) image tensors: H2D copies and the D2H loss read are inside
 the timed region.  `roofline` is for the dominant convolution kernel, timed live with CUDA events on the
 launching stream in a second timed region of the same K steps (the headline region carries no per-kernel events).
+`--dump-outputs DIR` writes what the last headline step computed (see dump_outputs) as DIR/<name>.npy; the inputs are
+seeded, so two builds run with the same arguments can be compared output for output.
 
 Comparison legs (measurement infrastructure, baseline/ref_runner.py):
   * `cpu_baseline` / `--impl reference`: the UNMODIFIED reference (`$COUNCIL_REF_DIR` -> /root/reference -> baseline/_ref; else the
     oracle port, `kind: "port"`) on the host cores, on a bounded sample of the workload (batch 1 -- the batch really run is
     printed), with the thread count chosen by a sweep at THIS workload (host core count printed);
-  * `gpu_library_baseline` (and `--impl reference-gpu`): the same unmodified reference on the same B200 under stock
+  * `gpu_library_baseline` (and `--impl reference-gpu`): the same unmodified reference on the same GPU under stock
     PyTorch + cuDNN at the workload's full batch (train.py:241-251 path, cudnn.deterministic as train.py:61, plus a
     cudnn.benchmark number) -- the comparator SURVEY.md 2.1 names.
 Before timing, the first step of our arm is checked against the reference's golden losses for the workload (1e-3).
@@ -65,8 +67,38 @@ def synth(batch, size, seed):
     return torch.rand(batch, 3, size, size, generator=g) * 2 - 1, torch.rand(batch, 3, size, size, generator=g) * 2 - 1
 
 
+DUMP_SAMPLE = 1 << 19  # parameters kept per network member (a fixed seeded sample of larger members)
+
+
+def dump_outputs(trainer, out_dir, n_members):
+    """What one training step hands its caller: the per-member total losses of the three updates (float64) and the updated
+    parameters of every network member (float32: the state_dict tensors flattened and concatenated in sorted key order; a
+    fixed seeded sample of DUMP_SAMPLE elements when a member is larger).  At most 64 MB in all."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {'loss_gen_total': trainer.loss_gen_total_s, 'loss_dis_total': trainer.loss_dis_total_s}
+    if getattr(trainer, 'do_dis_council', False):
+        arrays['loss_dis_council_total'] = trainer.loss_dis_council_total_s
+    arrays = {k: np.array([float(v) for v in vals], dtype=np.float64) for k, vals in arrays.items()}
+    fams = ['gen', 'dis'] + (['dis_council'] if getattr(trainer, 'do_dis_council', False) else [])
+    nets = ['%s_%s' % (f, d) for f in fams for d in ('a2b', 'b2a')]
+    per_member = min(DUMP_SAMPLE, (60 << 20) // (4 * len(nets) * n_members))
+    for name in nets:
+        for i, member in enumerate(getattr(trainer, name + '_s')):
+            sd = member.state_dict()
+            flat = torch.cat([sd[k].detach().reshape(-1).float().cpu() for k in sorted(sd)]).numpy()
+            if flat.size > per_member:
+                idx = np.sort(np.random.default_rng(1234).choice(flat.size, per_member, replace=False))
+                flat = flat[idx]
+            arrays['%s_%d_params' % (name, i)] = flat
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= 64 << 20, total
+    for k, a in arrays.items():
+        np.save(os.path.join(out_dir, k + '.npy'), a)
+
+
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     Q = 'clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,' \
         'clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap'
@@ -211,7 +243,8 @@ def main():
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-gpu-baseline', action='store_true')
     ap.add_argument('--no-parity-check', action='store_true')
-    ap.add_argument('--tc', type=int, default=1, help='0: SIMT fp32 kernels only, 1: tcgen05 TF32 where supported')
+    ap.add_argument('--tc', type=int, default=1, help='0: SIMT fp32 kernels only, 1: TF32 tensor-core kernels where supported')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None, help='write the outputs of the last timed step as DIR/<name>.npy')
     args = ap.parse_args()
     assert args.warmup >= 0 and args.steps >= 1
     rank = int(os.environ.get('RANK', '0'))
@@ -317,6 +350,8 @@ def main():
     l0 = ops.launch_count()
     ms = timed(lambda: step(xa_d, xb_d), args.steps)   # the headline timed region: nothing but the step's own launches in the stream
     launches = ops.launch_count() - l0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(trainer, args.dump_outputs, n_members)
     # second timed region of the same K steps with a CUDA-event pair around every convolution / HBM-pass launch (per-kernel averages for
     # the roofline): ~800 event records per step cost host time (the 128x128 configuration is launch-bound) and sit between kernels that
     # would otherwise overlap their launch, so they are kept out of the headline region; shares are taken against THIS region's time

@@ -1,4 +1,4 @@
-"""Build libcouncil_b200.so in-tree with nvcc for sm_100a (no torch dependency, plain C ABI)."""
+"""Build libcouncil_b200.so in-tree with nvcc for sm_90a (no torch dependency, plain C ABI)."""
 from __future__ import annotations
 
 import os
@@ -8,8 +8,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libcouncil_b200.so')
-SOURCES = ['api.cu', 'conv_simt.cu', 'conv_tc.cu', 'norm.cu', 'pointwise.cu', 'losses.cu', 'norm_coop.cu', 'conv_img.cu', 'head_fused.cu', 'conv_small.cu', 'augment.cu']
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+SOURCES = ['api.cu', 'conv_simt.cu', 'conv_tc.cu', 'norm.cu', 'pointwise.cu', 'losses.cu', 'norm_coop.cu', 'head_fused.cu', 'conv_small.cu', 'augment.cu']
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '--use_fast_math=false', '-Xcompiler', '-fPIC']
 
 
@@ -49,7 +49,7 @@ def build(force=False, verbose=False):
         if verbose:
             print(out)
         objs.append(obj)
-    cmd = [nvcc, '-shared', '-gencode', 'arch=compute_100a,code=sm_100a', '-o', LIB] + objs
+    cmd = [nvcc, '-shared', '-gencode', 'arch=compute_90a,code=sm_90a', '-o', LIB] + objs
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError('link failed:\n' + r.stdout)

@@ -130,17 +130,8 @@ extern "C" int cg_device_info(int* sm_count, int* cc_major, int* cc_minor) {
 extern "C" int cg_set_tensor_core_mode(int mode) {
     int prev = g_tc_mode;
     g_tc_mode = mode == 1 ? 7 : (mode & 7);  // 1 = everything; otherwise a bit mask: 1 forward, 2 data gradient, 4 weight gradient
-    // A/B switches: 8 = no CTA-pair (cta_group::2) kernels at all, 16 = none for 128-wide tiles, 32 = ALSO for 64-wide tiles, 64 = ALSO in the weight gradient
-    g_pair_mode = (mode & 8) ? 0 : (1 | ((mode & 16) ? 0 : 2) | ((mode & 32) ? 4 : 0) | ((mode & 64) ? 8 : 0));  // 64 = CTA pairs in wgrad too
-    g_wgrad_xm = (mode & 128) ? 0 : 1;  // 128 = no x-on-M weight gradient for <= 64 output channels
-    g_wgrad_2cta = ((mode >> 16) & 1) ? 0 : 1;  // bit 16: one weight-gradient CTA per SM (default: two co-resident CTAs)
-    g_wgrad_xm2 = ((mode >> 18) & 1) ? 0 : 1;   // bit 18: one x-on-M weight-gradient CTA per SM
-    g_fwd_2cta = ((mode >> 17) & 1) ? 0 : 1;    // bit 17: one forward / dgrad CTA per SM for tiles <= 64 wide (default: two co-resident)
-    g_img_path = ((mode >> 19) & 1) ? 0 : 1;    // bit 19: image-side layers on the older paths (TMA im2col forward, explicit patch matrix weight gradient)
-    g_epi_coalesce = ((mode >> 20) & 1) ? 0 : (((mode >> 21) & 1) ? 2 : 1);  // bit 20: accumulator-layout epilogue stores everywhere; bit 21: the coalescing patch on the wide tiles too
     g_small_bn = ((mode >> 23) & 1) ? 0 : 1;  // bit 23: keep the widest N tile even when the launch has fewer tiles than SMs
-    g_pdl = ((mode >> 22) & 1) ? 1 : (((mode >> 24) & 1) ? 2 : 0);  // bit 24: PDL for the helper kernels only  // bit 22: programmatic dependent launch (wins on launch-bound small maps, loses ~2 % at 256x256 x 8)
-    g_pair_cap = (mode >> 8) & 0xff;  // bits 8..15: cap on the number of CTA pairs launched (0 = as many as are co-resident)
+    g_pdl = ((mode >> 22) & 1) ? 1 : (((mode >> 24) & 1) ? 2 : 0);  // bit 22: programmatic dependent launch; bit 24: for the helper kernels only
     return prev;
 }
 
@@ -165,7 +156,6 @@ extern "C" size_t cg_conv_workspace_bytes(const cg_conv_geom* g, int which) {
     const bool patch_fwd = which == 0 && (g_tc_mode & 1) && patch_path(*g) && g->KH * g->KW >= 16;
     if (which == 2 && small_wgrad_supported(*g)) return small_ws(*g, 2);
     if (which == 1 && small_dgrad_supported(*g)) return small_ws(*g, 1);
-    if (which == 2 && (g_tc_mode & 4) && img_wgrad_supported(*g)) return img_wgrad_ws(*g);
     const bool patch_wgrad = which == 2 && (g_tc_mode & 4) && patch_path(*g);
     if (patch_fwd || patch_wgrad) {
         cg_conv_geom p = patch_geom(*g);
@@ -194,9 +184,8 @@ extern "C" int cg_conv_fwd(const cg_conv_geom* g, const float* x, const float* w
     if (int rc = validate_geom(*g)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     if (small_fwd_supported(*g, act)) return small_conv_fwd(*g, x, w, bias, y, st);
-    if ((g_tc_mode & 1) && img_fwd_supported(*g, act)) return img_conv_fwd(*g, x, w, bias, y, act, slope, st);
     // forward: the patch matrix pays off when there are many taps (7x7: 49, 4x4: 16); the 3x3 pair layer is faster
-    // straight through TMA im2col with 32-byte rows (measured 3.1 ms vs 4.7 ms at B=40, 256x256)
+    // straight through TMA im2col with 32-byte rows (9 taps: the patch matrix would be nearly as large as the map it replaces)
     if ((g_tc_mode & 1) && patch_path(*g) && g->KH * g->KW >= 16 && act != CG_ACT_TANH) {
         size_t need = cg_conv_workspace_bytes(g, 0);
         if (need > ws_bytes) {
@@ -238,7 +227,6 @@ extern "C" int cg_conv_wgrad(const cg_conv_geom* g, const float* x, const float*
     if (int rc = validate_geom(*g)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     if (small_wgrad_supported(*g)) return small_conv_wgrad(*g, x, dy, dw, db, ws, ws_bytes, st);
-    if ((g_tc_mode & 4) && img_wgrad_supported(*g)) return img_conv_wgrad(*g, x, dy, dw, db, ws, ws_bytes, st);
     if ((g_tc_mode & 4) && patch_path(*g)) {
         size_t need = cg_conv_workspace_bytes(g, 2);
         if (need > ws_bytes) {

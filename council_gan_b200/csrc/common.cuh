@@ -1,4 +1,4 @@
-// Shared helpers for libcouncil_b200.so (sm_100a only).
+// Shared helpers for libcouncil_b200.so (sm_90a).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -14,14 +14,7 @@ void set_error(const char* fmt, ...);
 extern std::atomic<uint64_t> g_launches;
 // kernel-selection switches of cg_set_tensor_core_mode: per calling THREAD (like cg_last_error), not process-global
 extern thread_local int g_tc_mode;
-extern thread_local int g_pair_mode;
-extern thread_local int g_pair_cap;
-extern thread_local int g_wgrad_xm;
-extern thread_local int g_wgrad_2cta;
-extern thread_local int g_fwd_2cta;
-extern thread_local int g_epi_coalesce;
 extern thread_local int g_small_bn;
-extern thread_local int g_wgrad_xm2;
 
 constexpr int CG_MAX_DEVICES = 64;
 inline int current_device() {
@@ -59,13 +52,12 @@ static inline int cdiv(long a, long b) { return (int)((a + b - 1) / b); }
 // ---- programmatic dependent launch (PDL) --------------------------------------------------------------------------------------------
 // A training step is ~670 short-to-medium kernels in one stream.  Every kernel of this library (a) lets its successor start launching
 // at once (griddepcontrol.launch_dependents as its first instruction: CTAs of the next kernel are scheduled as SM resources free up and run
-// their on-chip prologue -- barrier init, TMEM allocation, tensor-map prefetch) and (b) executes griddepcontrol.wait before it touches
+// their on-chip prologue -- barrier init, tensor-map prefetch) and (b) executes griddepcontrol.wait before it touches
 // global memory: that blocks until the WHOLE preceding grid has completed and its writes are visible, so the data dependences are
 // exactly those of plain stream order (every kernel waits, so completion is transitive along the stream).  Kernels of other libraries
 // (NCCL, memsets, copies) are launched without the attribute and keep full stream serialisation on both sides.
-// Measured (visit N, alternating runs on one box): 128x128 council of 2 batch 1: 9.71 -> 9.34 ms per step; 256x256 council of 4 batch 8:
-// 79.0 -> 80.7 ms -- early-scheduled dependents cost more than the launch gaps they hide once kernels are long.  The attribute is therefore
-// OFF unless mode bit 22 asks for it (the trainer does on small maps: COUNCIL_PDL=auto|0|1).
+// Early-scheduled dependents cost more than the launch gaps they hide once kernels are long, so the attribute is OFF unless mode
+// bit 22 asks for it (the trainer does on small, launch-bound maps: COUNCIL_PDL=auto|0|1).
 extern thread_local int g_pdl;
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -123,7 +115,7 @@ size_t colsum_ws(int G, long rows, int C);
 int pool2x2_sum(const float* d_up, float* dx, const float* addend, const float* mask_src, float mask_slope,
                 long N, int H, int W, int C, cudaStream_t st);
 
-// ---- tcgen05 TF32 implicit-GEMM convolutions (conv_tc.cu) ----
+// ---- TF32 tensor-core implicit-GEMM convolutions (conv_tc.cu) ----
 bool tc_fwd_supported(const cg_conv_geom& g);
 int tc_conv_fwd(const cg_conv_geom& g, const float* x, const float* w, const float* bias, float* y,
                 int act, float slope, void* ws, size_t ws_bytes, cudaStream_t st, float* stats_part = nullptr);
@@ -140,18 +132,8 @@ size_t tc_wgrad_ws(const cg_conv_geom& g);
 int tc_conv_wgrad(const cg_conv_geom& g, const float* x, const float* dy, float* dw, void* ws, size_t ws_bytes,
                   cudaStream_t st);
 
-int tc_encode_mn_map(CUtensorMap* map, const float* t, long rows, int C, int kp);
-int tc_encode_store_map(CUtensorMap* map, float* t, long rows, int C, int box_rows);
 int tc_sm_count();
 void tc_map_cache_stats(uint64_t* hits, uint64_t* misses);
-
-// ---- image-side convolutions (<= 8 input lanes, 64 output channels) with patches built in shared memory (conv_img.cu) ----
-bool img_fwd_supported(const cg_conv_geom& g, int act);
-int img_conv_fwd(const cg_conv_geom& g, const float* x, const float* w, const float* bias, float* y, int act, float slope, cudaStream_t st);
-bool img_wgrad_supported(const cg_conv_geom& g);
-size_t img_wgrad_ws(const cg_conv_geom& g);
-int img_conv_wgrad(const cg_conv_geom& g, const float* x, const float* dy, float* dw, float* db, void* ws, size_t ws_bytes, cudaStream_t st);
-extern thread_local int g_img_path;
 
 // ---- vector-shaped layers (512 -> 1 patch heads, the MLP's wide output layer) as streaming fp32 kernels (conv_small.cu) ----
 bool small_fwd_supported(const cg_conv_geom& g, int act);

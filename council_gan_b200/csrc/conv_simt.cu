@@ -1,7 +1,7 @@
 // SIMT fp32 implicit-GEMM convolutions: forward, data gradient, weight gradient.
 //
 // These are the exact-fp32 kernels of the library.  They serve (a) the layers that do not qualify
-// for the tcgen05 path (3/6/12/1-channel image-side layers, the MLP), (b) as the on-device
+// for the tensor-core path (maps with < 128 pixels per member, the small MLP layers), (b) as the on-device
 // reference the tensor-core kernels are verified against (cg_set_tensor_core_mode(0)).
 //
 // Reference call sites replaced: nn.Conv2d forward (networks.py:513,516) and its autograd

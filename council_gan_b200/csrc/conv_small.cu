@@ -6,9 +6,8 @@
 //       wgrad     dw[c]     = sum_px dy[px] * x[px][c],  db = sum_px dy[px]     two-phase, fixed order
 //   * the data gradient of the last MLP layer (nn.Linear(256, 5888), networks.py:438): an 8 x 5888 x 256 product per member
 //
-// Through the generic 64x64x16 SIMT tiles these took 0.3-0.5 ms per launch (N = 1 wastes 63/64 of a tile; the MLP gradient
-// has 5888-long reductions and 8 rows): ~2.2 ms per step (launch list profiles/r02_runF_launches_bench.csv).  They are
-// HBM-trivial: 67 MB at the largest call.
+// The generic 64x64x16 SIMT tiles fit them badly (N = 1 wastes 63/64 of a tile; the MLP gradient has 5888-long reductions and
+// 8 rows).  They are HBM-trivial: 67 MB at the largest call.
 #include "common.cuh"
 
 namespace cg {

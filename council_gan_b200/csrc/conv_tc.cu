@@ -1,17 +1,16 @@
-// tcgen05 TF32 implicit-GEMM convolution for sm_100a.
+// TF32 implicit-GEMM convolution for sm_90a (TMA + mbarrier pipeline, warpgroup MMA).
 //
-//   D[128 pixels x BN couts] (fp32, TMEM) += A[128 x 32] (im2col tile of x, smem) * B[BN x 32] (weights, smem)
+//   D[128 pixels x BN couts] (fp32, registers) += A[128 x 32] (im2col tile of x, smem) * B[BN x 32] (weights, smem)
 //
 // * A tiles are gathered by TMA in IM2COL mode straight from the channels-last activation tensor
 //   [G*B][H][W][Cin]: the zero padding of nn.ZeroPad2d (networks.py:473-474) is the TMA out-of-bound
 //   fill, the stride is the TMA traversal stride -- there is no pad kernel and no im2col buffer.
 // * B tiles are 2-D TMA boxes of the OHWI weight matrix [G*Cout][KH*KW*Cin] (K-major).
-// * both land in shared memory in the 128-byte swizzled K-major layout tcgen05.mma reads; operands are
-//   fp32 in HBM, converted to TF32 by the tensor map data type; accumulation is fp32 in tensor memory.
-// * warp-specialised persistent CTAs (one per SM): warp 0 = TMA producer, warp 1 = MMA issuer (+TMEM
-//   allocator), warps 2..5 = epilogue (tcgen05.ld -> bias / activation / addend / mask -> global).
-//   smem ring of STAGES (A,B) tiles with full/empty mbarriers; two TMEM accumulator stages so the epilogue
-//   of tile i overlaps the mainloop of tile i+1.
+// * both land in shared memory in the 128-byte swizzled K-major layout wgmma reads; operands are
+//   fp32 in HBM, converted to TF32 by the tensor map data type; accumulation is fp32 in registers.
+// * warp-specialised persistent CTAs (one per SM): one producer thread issues the TMA loads, two consumer
+//   warpgroups (64 pixel rows each) issue the MMAs and run the epilogue (bias / activation / addend / mask -> global).
+//   smem ring of stages of (A,B) tiles with full/empty mbarriers.
 // * all N council members are one launch: the member index is folded into the tensor-map coordinates
 //   (image index g*B+n for A, row g*Cout+co for B), i.e. a grouped GEMM over the council.
 //
@@ -20,11 +19,8 @@
 // own im2col bounding box and a strided output mapping (see tc_conv_dgrad).
 //
 // Kernels in this file (host dispatch at the bottom of each section):
-//   conv_tc_kernel<32|8>  forward / data gradient, one CTA per SM (tcgen05.mma.cta_group::1)
-//   conv_tc2_kernel       the same for 128/256-wide tiles as CTA pairs (cta_group::2, M = 256 over two SMs)
-//   wgrad_tc_kernel       weight gradient, cout on M, MN-major operands straight from the NHWC tensors
-//   wgrad_xm_kernel       weight gradient with x on M for <= 64 output channels
-//   wgrad_tc2_kernel      CTA-pair weight gradient (measured slower; behind a cg_set_tensor_core_mode switch)
+//   conv_tc_kernel<BK, BN>  forward / data gradient
+//   wgrad_tc_kernel<BM, BN> weight gradient (MN-major operands transposed in shared memory, then wgmma)
 //
 // Reference call sites replaced: nn.Conv2d forward (networks.py:513,516) and cuDNN dgrad via autograd.
 #include "common.cuh"
@@ -54,15 +50,7 @@ static int sm_count_now() {
     if (!g_sm_count_dev[dev]) cudaDeviceGetAttribute(&g_sm_count_dev[dev], cudaDevAttrMultiProcessorCount, dev);
     return g_sm_count_dev[dev];
 }
-thread_local int g_pair_cap = 0;
-thread_local int g_wgrad_xm = 1;  // x-on-M weight gradient for <= 64 output channels
-thread_local int g_wgrad_2cta = 1;  // two co-resident weight-gradient CTAs per SM (run 44: -14..-33 % on the >= 128-channel layers)
-thread_local int g_wgrad_xm2 = 1;   // ... also for the x-on-M kernel
 thread_local int g_small_bn = 1;  // narrower N tiles when a launch has fewer tiles than SMs (mode bit 23 clears it)
-thread_local int g_epi_coalesce = 1;  // epilogue stores through the per-warp patch (full sectors); bit 20 of the mode clears it
-thread_local int g_fwd_2cta = 1;    // two co-resident forward / data-gradient CTAs per SM for tiles <= 64 channels wide (run 46: -1.4 ms/step)
-thread_local int g_pair_mode = 3;  // bit 0: 256-wide tiles, bit 1: 128-wide, bit 2: 64-wide (measured slower than single CTAs: off),
-                      // bit 3: weight gradient (MN-major operands: measured 15-20 % slower than single CTAs: off)  // cta_group::2 kernels for 256-wide layers (cg_set_tensor_core_mode bit 8 clears it for A/B runs)
 static int g_driver_version = 0;
 static std::once_flag g_once;
 
@@ -137,13 +125,10 @@ static void init_driver() {
 // ------------------------------------------------------------------------------------------------
 // kernel
 // ------------------------------------------------------------------------------------------------
-constexpr int TC_BM = 128;          // pixels per tile (TMEM lanes)
+constexpr int TC_BM = 128;          // pixels per tile
 constexpr int TC_BK = 32;           // fp32 channels per stage = one 128-byte swizzle row
-constexpr int TC_THREADS = 192;     // 6 warps: 0 TMA producer, 1 MMA issuer, 2..5 epilogue (TMEM lane quadrant = warp id % 4)
-// Measured both ways: giving the two single-thread roles the HIGHEST warp ids (4, 5; epilogue 0..3) is ~4 % slower
-// (102.2 vs 98.0 ms per step), so they keep ids 0 and 1.
-constexpr int TC_PRODUCER_WARP = 0;
-constexpr int TC_MMA_WARP = 1;
+constexpr int TC_THREADS = 384;     // warpgroup 0: TMA producer (one thread); warpgroups 1, 2: wgmma + epilogue of tile rows 0..63 / 64..127
+constexpr int TC_MAX_STAGES = 12;
 constexpr int TC_MAX_CLASSES = 4;   // stride-2 dgrad: one im2col map per output parity class
 
 struct TcClass {
@@ -155,8 +140,6 @@ struct TcClass {
 };
 struct TcParams {
     CUtensorMap bmap;               // weights [rows][Ktot_class] 2-D
-    const float* w_base;            // (host) what bmap was encoded over, so the CTA-pair launch can re-encode it with 128-row boxes
-    long w_rows, w_ktot;
     TcClass cls[TC_MAX_CLASSES];
     int ncls;
     int G, xg_images;               // groups; images per group in the activation map (0: shared input)
@@ -164,8 +147,8 @@ struct TcParams {
     int Cin, Cout, KH, KW, stride;  // KH,KW: taps per class
     int bn;                         // N tile
     int bk;                         // K elements per stage: 32 (128-byte swizzled rows) or 8 (32-byte rows, Cin = 8)
-    int cps;                        // K chunks per pipeline stage (small-N layers batch several: the MMA issue loop is latency bound)
-    int n_store;                    // output channels actually stored per N tile (== bn except the 8-lane image gradient)
+    int cps;                        // K chunks per pipeline stage
+    int n_store;                    // output channels actually stored per N tile (== bn except the narrow image / head outputs)
     int out_H, out_W, out_sh, out_sw;  // full output spatial size and class strides
     int w_rows_per_group;           // weight rows per group (ncls * Cout for dgrad classes)
     float* y; const float* bias; const float* addend; const float* mask_src;
@@ -173,125 +156,46 @@ struct TcParams {
     long stats_gbc;                 // G*B*Cout
     int act; float slope;
     int stages;
-    int coalesce;                   // epilogue leaves through the per-warp shared-memory patch with full-sector global accesses
 };
 
-// Epilogue store of one 32-row x 32-column accumulator block (lane = pixel row, v = its 32 channels, bias already added) with
-// FULL-sector global accesses.  In the accumulator layout a warp-wide float4 store touches 32 different pixels, 16 bytes each:
-// 32 half-written sectors per instruction, which capped the store-heavy layers near 2 TB/s (profiles/r02_summary.md).  Here the
-// block goes through a 2 KB per-warp shared-memory patch, 16 columns at a time (64-byte rows, float4 index XOR-swizzled by
-// (row >> 1) & 3: conflict-free for the row-wise writes and for the reads below), after which four consecutive lanes own 64
-// contiguous bytes of one pixel -- for the stores and for the residual (addend) / activation-mask loads of the data gradient alike.
-// out_off: element offset of this lane's pixel row at the block's first column, or -1 when the row is not stored.
-__device__ __forceinline__ void epilogue_store_coalesced(const float (&v)[32], float4* patch, int lane, long out_off, float* __restrict__ y,
-                                                         const float* __restrict__ addend, const float* __restrict__ mask_src, int act,
-                                                         float slope) {
-    const int wsw = (lane >> 1) & 3, c4 = lane & 3;
-    long offs[4];
-#pragma unroll
-    for (int i = 0; i < 4; i++) offs[i] = __shfl_sync(0xffffffffu, out_off, i * 8 + (lane >> 2));
-    // every residual / mask load of the block is issued before the shared-memory round trip (one exposed latency, not eight)
-    float4 av[2][4], mv[2][4];
-    if (addend) {
-#pragma unroll
-        for (int half = 0; half < 2; half++)
-#pragma unroll
-            for (int i = 0; i < 4; i++)
-                av[half][i] = offs[i] >= 0 ? __ldg(reinterpret_cast<const float4*>(addend + offs[i] + half * 16 + c4 * 4)) : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    if (mask_src) {
-#pragma unroll
-        for (int half = 0; half < 2; half++)
-#pragma unroll
-            for (int i = 0; i < 4; i++)
-                mv[half][i] = offs[i] >= 0 ? __ldg(reinterpret_cast<const float4*>(mask_src + offs[i] + half * 16 + c4 * 4)) : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-#pragma unroll
-    for (int half = 0; half < 2; half++) {
-        __syncwarp();
-#pragma unroll
-        for (int j = 0; j < 4; j++)
-            patch[lane * 4 + (j ^ wsw)] = make_float4(v[16 * half + 4 * j], v[16 * half + 4 * j + 1], v[16 * half + 4 * j + 2], v[16 * half + 4 * j + 3]);
-        __syncwarp();
-#pragma unroll
-        for (int i = 0; i < 4; i++) {
-            const int r = i * 8 + (lane >> 2);
-            float4 o = patch[r * 4 + (c4 ^ ((r >> 1) & 3))];
-            if (offs[i] < 0) continue;
-            if (addend) {
-                const float4 a = av[half][i];
-                o.x += a.x; o.y += a.y; o.z += a.z; o.w += a.w;
-            }
-            if (mask_src) {
-                const float4 a = mv[half][i];
-                o.x *= a.x > 0.f ? 1.f : slope; o.y *= a.y > 0.f ? 1.f : slope;
-                o.z *= a.z > 0.f ? 1.f : slope; o.w *= a.w > 0.f ? 1.f : slope;
-            } else if (act == CG_ACT_RELU) {
-                o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f);
-            } else if (act == CG_ACT_LRELU) {
-                o.x = o.x > 0.f ? o.x : o.x * slope; o.y = o.y > 0.f ? o.y : o.y * slope;
-                o.z = o.z > 0.f ? o.z : o.z * slope; o.w = o.w > 0.f ? o.w : o.w * slope;
-            }
-            *reinterpret_cast<float4*>(y + offs[i] + half * 16 + c4 * 4) = o;
-        }
-    }
-}
-
-template <int BK>
-__global__ void __launch_bounds__(TC_THREADS, 2) conv_tc_kernel(const __grid_constant__ TcParams p) {
+// Persistent CTAs (one per SM) walk the tiles (group, class, N tile, pixel tile).  The producer thread streams (A, B) chunks
+// through a ring of `stages` shared-memory slots guarded by full / empty mbarriers; each consumer warpgroup multiplies its 64
+// pixel rows of A with the whole B tile (wgmma, accumulators in registers), releases a slot as soon as the MMAs that read it
+// have retired, and runs the epilogue straight from registers while the producer already fills the slots of the next tile.
+template <int BK, int BN>
+__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_constant__ TcParams p) {
     pdl_trigger();
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int a_bytes = TC_BM * BK * 4;                       // one K chunk of A
-    const int b_bytes = ((p.bn * BK * 4) + 1023) & ~1023;    // one K chunk of B (slot size)
-    const int stage_bytes = p.cps * (a_bytes + b_bytes);       // [A_0..A_cps-1][B_0..B_cps-1]
-    const int tx_chunk = a_bytes + p.bn * BK * 4;
+    const int wg = __shfl_sync(0xffffffffu, threadIdx.x >> 7, 0), tid = threadIdx.x & 127;  // warp-uniform for the compiler
+    constexpr int a_bytes = TC_BM * BK * 4;                      // one K chunk of A
+    constexpr int b_bytes = ((BN * BK * 4) + 1023) & ~1023;     // one K chunk of B (slot size)
+    const int stage_bytes = p.cps * (a_bytes + b_bytes);         // [A_0..A_cps-1][B_0..B_cps-1]
+    constexpr int tx_chunk = a_bytes + BN * BK * 4;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * stage_bytes);
     uint64_t* empty_bar = full_bar + p.stages;
-    uint64_t* tfull_bar = empty_bar + p.stages;
-    uint64_t* tempty_bar = tfull_bar + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-    float* stat_smem = reinterpret_cast<float*>(tmem_slot + 4);  // 4 x (32 x 36) floats, only carved when p.stats
-    float4* store_patch = reinterpret_cast<float4*>(stat_smem + (p.stats ? 4 * 32 * 36 : 0));  // 4 x 2 KB, only carved when p.coalesce
 
     const int MT = (p.B * p.P * p.Q + TC_BM - 1) / TC_BM;  // pixel tiles per (group, class)
-    const int NT = (p.Cout + p.bn - 1) / p.bn;
+    const int NT = (p.Cout + BN - 1) / BN;
     const int tiles = p.G * p.ncls * NT * MT;
     const int kchunks = (p.Cin + BK - 1) / BK;  // a partial last chunk reads zero-filled channels
     const int kiters = p.KH * p.KW * kchunks;
-    const int tmem_cols = 2 * p.bn < 32 ? 32 : 2 * p.bn;
 
-    if (warp == TC_PRODUCER_WARP && lane == 0) {
+    if (threadIdx.x == 0) {
         prefetch_tmap(&p.bmap);
         for (int c = 0; c < p.ncls; c++) prefetch_tmap(&p.cls[c].amap);
-    }
-    if (warp == TC_MMA_WARP) {
-        if (lane == 0) {
-            for (int s = 0; s < p.stages; s++) {
-                mbar_init(&full_bar[s], 1);
-                mbar_init(&empty_bar[s], 1);
-            }
-            for (int a = 0; a < 2; a++) {
-                mbar_init(&tfull_bar[a], 1);
-                mbar_init(&tempty_bar[a], 128);
-            }
-            fence_barrier_init();
+        for (int s = 0; s < p.stages; s++) {
+            mbar_init(&full_bar[s], 1);
+            mbar_init(&empty_bar[s], 2);  // one arrival per consumer warpgroup
         }
-        __syncwarp();
-        // TMEM allocation (power of two >= 32 columns), whole warp
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(tmem_cols));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
+        fence_barrier_init();
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    pdl_wait();  // on-chip prologue done (barriers, TMEM): from here on the kernel reads what its predecessors in the stream wrote
+    pdl_wait();  // on-chip prologue done: from here on the kernel reads what its predecessors in the stream wrote
 
-    if (warp == TC_PRODUCER_WARP) {
+    if (wg == 0) {
         // ===================== TMA producer =====================
-        if (lane == 0) {
+        if (tid == 0) {
             int stage = 0;
             uint32_t phase = 0;
             for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
@@ -309,7 +213,7 @@ __global__ void __launch_bounds__(TC_THREADS, 2) conv_tc_kernel(const __grid_con
                 int n_coord = g * p.xg_images + img;
                 int w_coord = cl.w0 + qq * p.stride;
                 int h_coord = cl.h0 + pp * p.stride;
-                int wrow = g * p.w_rows_per_group + cl.wrow_off + nt * p.bn;
+                int wrow = g * p.w_rows_per_group + cl.wrow_off + nt * BN;
                 int kh = 0, kw = 0, kc = 0;
                 for (int k0 = 0; k0 < kiters; k0 += p.cps) {
                     const int n = kiters - k0 < p.cps ? kiters - k0 : p.cps;
@@ -327,489 +231,115 @@ __global__ void __launch_bounds__(TC_THREADS, 2) conv_tc_kernel(const __grid_con
                 }
             }
         }
-    } else if (warp == TC_MMA_WARP) {
-        // ===================== MMA issuer =====================
-        if (lane == 0) {
-            const uint32_t idesc = make_idesc_tf32(p.bn);
-            // descriptor without the start address (same for every chunk of this launch)
-            const uint64_t desc_hi = (BK == 32 ? make_kmajor_sw128_desc(0) : make_kmajor_sw32_desc(0));
-            int stage = 0;
-            uint32_t phase = 0;
-            int acc = 0;
-            uint32_t acc_phase = 0;
-            for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
-                mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * p.bn);
-                for (int k0 = 0; k0 < kiters; k0 += p.cps) {
-                    const int n = kiters - k0 < p.cps ? kiters - k0 : p.cps;
-                    mbar_wait(&full_bar[stage], phase);
-                    tc_fence_after();
-                    const uint32_t sa = smem_u32(smem + (size_t)stage * stage_bytes);
-                    const uint32_t sb = sa + p.cps * a_bytes;
-                    for (int j = 0; j < n; j++) {
-                        const uint64_t adesc = desc_hi | (uint64_t)(((sa + j * a_bytes) & 0x3FFFF) >> 4);
-                        const uint64_t bdesc = desc_hi | (uint64_t)(((sb + j * b_bytes) & 0x3FFFF) >> 4);
+        return;
+    }
+
+    // ===================== MMA + epilogue (consumer warpgroups) =====================
+    const int cw = wg - 1;                                   // tile rows 64 cw .. 64 cw + 63
+    const int warp4 = tid >> 5, lane = tid & 31;
+    const int row0 = cw * 64 + warp4 * 16 + (lane >> 2);     // this thread's accumulator rows: row0, row0 + 8
+    const int cq = 2 * (lane & 3);                           // ... and columns 8 j + cq, 8 j + cq + 1
+    const uint64_t desc0 = BK == 32 ? make_kmajor_sw128_desc(0) : make_kmajor_sw32_desc(0);
+    float acc[BN / 2];
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+        int mt = t % MT;
+        int r = t / MT;
+        int nt = r % NT;
+        r /= NT;
+        int c = r % p.ncls;
+        int g = r / p.ncls;
+        const TcClass& cl = p.cls[c];
+        int prev = -1;
+        for (int k0 = 0; k0 < kiters; k0 += p.cps) {
+            const int n = kiters - k0 < p.cps ? kiters - k0 : p.cps;
+            mbar_wait(&full_bar[stage], phase);
+            const uint32_t sa = smem_u32(smem + (size_t)stage * stage_bytes) + cw * (64 * BK * 4);
+            const uint32_t sb = smem_u32(smem + (size_t)stage * stage_bytes) + p.cps * a_bytes;
+            wgmma_fence();
+            for (int j = 0; j < n; j++) {
+                const uint64_t adesc = desc0 | (uint64_t)(((sa + j * a_bytes) & 0x3FFFF) >> 4);
+                const uint64_t bdesc = desc0 | (uint64_t)(((sb + j * b_bytes) & 0x3FFFF) >> 4);
 #pragma unroll
-                        for (int kk = 0; kk < BK / 8; kk++) {
-                            // advance 8 tf32 (32 bytes) along K inside the swizzled row: +2 in the 16-byte address field
-                            umma_tf32(d_tmem, adesc + (uint64_t)(kk * 2), bdesc + (uint64_t)(kk * 2), idesc, (k0 | j | kk) != 0 ? 1u : 0u);
-                        }
-                    }
-                    umma_commit(&empty_bar[stage]);  // frees the smem slot when these MMAs retire
-                    if (++stage == p.stages) { stage = 0; phase ^= 1; }
-                }
-                umma_commit(&tfull_bar[acc]);  // accumulator complete
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+                for (int kk = 0; kk < BK / 8; kk++)  // advance 8 tf32 (32 bytes) along K inside the swizzled row: +2 in the address field
+                    wgmma_tf32<BN>(acc, adesc + (uint64_t)(kk * 2), bdesc + (uint64_t)(kk * 2), (k0 | j | kk) != 0 ? 1 : 0);
             }
+            wgmma_commit();
+            wgmma_wait<1>();  // the MMAs of the previous stage have retired: its slot can be refilled
+            if (prev >= 0 && tid == 0) mbar_arrive(&empty_bar[prev]);
+            prev = stage;
+            if (++stage == p.stages) { stage = 0; phase ^= 1; }
         }
-    } else {
-        // ===================== epilogue (warps 2..5 -> TMEM lane quadrants 2,3,0,1) =====================
-        const int quad = warp & 3;
-        const int row = quad * 32 + lane;
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
-            int mt = t % MT;
-            int r = t / MT;
-            int nt = r % NT;
-            r /= NT;
-            int c = r % p.ncls;
-            int g = r / p.ncls;
-            const TcClass& cl = p.cls[c];
-            mbar_wait(&tfull_bar[acc], acc_phase);
-            tc_fence_after();
-            const int m = mt * TC_BM + row;      // < 2^31: B*P*Q pixels per member
-            const int pq = p.P * p.Q;
-            bool valid = m < p.B * pq;
-            long out_off = 0;
-            if (valid) {
+        wgmma_wait<0>();
+        wgmma_reg_fence(acc, BN / 2);
+        if (tid == 0) mbar_arrive(&empty_bar[prev]);
+
+        const int pq = p.P * p.Q;
+        long out_off[2];
+        bool valid[2];
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const int m = mt * TC_BM + row0 + 8 * h;  // < 2^31: B*P*Q pixels per member
+            valid[h] = m < p.B * pq;
+            out_off[h] = 0;
+            if (valid[h]) {
                 int img = m / pq;
                 int rem = m - img * pq;
                 int pp = rem / p.Q, qq = rem - pp * p.Q;
                 long pix = ((long)(g * p.B + img) * p.out_H + (pp * p.out_sh + cl.out_h0)) * p.out_W + (qq * p.out_sw + cl.out_w0);
-                out_off = pix * p.Cout + nt * p.n_store;
-            }
-            const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * p.bn);
-            if (p.n_store < 32) {
-                // narrow outputs (image-lane gradients, the 12-channel head): 16 accumulator columns, n_store stored
-                float v[32];
-                tmem_ld16(taddr, v);
-                if (valid) {
-#pragma unroll
-                    for (int j = 0; j < 16; j += 4) {
-                        if (j >= p.n_store) break;
-                        float4 o = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-                        if (p.bias) {
-                            const float* bp = p.bias + (long)g * p.Cout + j;
-                            o.x += __ldg(bp); o.y += __ldg(bp + 1); o.z += __ldg(bp + 2); o.w += __ldg(bp + 3);
-                        }
-                        if (p.addend) {
-                            float4 a = __ldg(reinterpret_cast<const float4*>(p.addend + out_off + j));
-                            o.x += a.x; o.y += a.y; o.z += a.z; o.w += a.w;
-                        }
-                        if (p.mask_src) {
-                            float4 a = __ldg(reinterpret_cast<const float4*>(p.mask_src + out_off + j));
-                            o.x *= a.x > 0.f ? 1.f : p.slope; o.y *= a.y > 0.f ? 1.f : p.slope;
-                            o.z *= a.z > 0.f ? 1.f : p.slope; o.w *= a.w > 0.f ? 1.f : p.slope;
-                        } else if (p.act != CG_ACT_NONE) {
-                            o.x = apply_act(o.x, p.act, p.slope); o.y = apply_act(o.y, p.act, p.slope);
-                            o.z = apply_act(o.z, p.act, p.slope); o.w = apply_act(o.w, p.act, p.slope);
-                        }
-                        *reinterpret_cast<float4*>(p.y + out_off + j) = o;
-                    }
-                }
-            } else
-            for (int c0 = 0; c0 < p.bn; c0 += 32) {
-                float v[32];
-                tmem_ld32(taddr + (uint32_t)c0, v);
-                if (p.stats) {
-                    // instance-norm statistics of the raw convolution output, fused here instead of a second pass over y.
-                    // Every tile lies inside one image (P*Q % 128 == 0) and this warp owns 32 of its rows: transpose the
-                    // 32x32 block through a private shared-memory patch (row stride 36 floats: conflict-free both ways) and
-                    // let lane j sum column j.
-                    float* patch = stat_smem + quad * (32 * 36);
-                    __syncwarp();
-#pragma unroll
-                    for (int j = 0; j < 8; j++)
-                        *reinterpret_cast<float4*>(patch + lane * 36 + 4 * j) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                    __syncwarp();
-                    float cs = 0.f, cq = 0.f;
-#pragma unroll
-                    for (int r = 0; r < 32; r++) {
-                        float e = patch[r * 36 + lane];
-                        cs += e;
-                        cq = fmaf(e, e, cq);
-                    }
-                    const int tiles_per_img = pq / TC_BM;
-                    const int img = (mt * TC_BM) / pq;
-                    const int chunk = ((c * tiles_per_img + (mt - img * tiles_per_img)) << 2) + quad;
-                    const long col = (long)(g * p.B + img) * p.Cout + nt * p.bn + c0 + lane;
-                    *reinterpret_cast<float2*>(p.stats + ((long)chunk * p.stats_gbc + col) * 2) = make_float2(cs, cq);
-                }
-                if (p.coalesce) {
-                    if (p.bias) {
-                        const float4* bp = reinterpret_cast<const float4*>(p.bias + (long)g * p.Cout + nt * p.bn + c0);
-#pragma unroll
-                        for (int j = 0; j < 8; j++) {
-                            float4 a = __ldg(bp + j);
-                            v[4 * j] += a.x; v[4 * j + 1] += a.y; v[4 * j + 2] += a.z; v[4 * j + 3] += a.w;
-                        }
-                    }
-                    epilogue_store_coalesced(v, store_patch + quad * 128, lane, valid ? out_off + c0 : -1, p.y, p.addend, p.mask_src, p.act, p.slope);
-                } else
-                if (valid) {
-                    if (p.bias) {
-                        const float4* bp = reinterpret_cast<const float4*>(p.bias + (long)g * p.Cout + nt * p.bn + c0);
-#pragma unroll
-                        for (int j = 0; j < 8; j++) {
-                            float4 a = __ldg(bp + j);
-                            v[4 * j] += a.x; v[4 * j + 1] += a.y; v[4 * j + 2] += a.z; v[4 * j + 3] += a.w;
-                        }
-                    }
-                    if (p.addend) {
-                        const float4* ap = reinterpret_cast<const float4*>(p.addend + out_off + c0);
-#pragma unroll
-                        for (int j = 0; j < 8; j++) {
-                            float4 a = __ldg(ap + j);
-                            v[4 * j] += a.x; v[4 * j + 1] += a.y; v[4 * j + 2] += a.z; v[4 * j + 3] += a.w;
-                        }
-                    }
-                    if (p.mask_src) {
-                        const float4* mp = reinterpret_cast<const float4*>(p.mask_src + out_off + c0);
-#pragma unroll
-                        for (int j = 0; j < 8; j++) {
-                            float4 a = __ldg(mp + j);
-                            v[4 * j] *= a.x > 0.f ? 1.f : p.slope; v[4 * j + 1] *= a.y > 0.f ? 1.f : p.slope;
-                            v[4 * j + 2] *= a.z > 0.f ? 1.f : p.slope; v[4 * j + 3] *= a.w > 0.f ? 1.f : p.slope;
-                        }
-                    } else if (p.act == CG_ACT_RELU) {
-#pragma unroll
-                        for (int j = 0; j < 32; j++) v[j] = fmaxf(v[j], 0.f);
-                    } else if (p.act == CG_ACT_LRELU) {
-#pragma unroll
-                        for (int j = 0; j < 32; j++) v[j] = v[j] > 0.f ? v[j] : v[j] * p.slope;
-                    }  // tanh only occurs on the narrow (<= 16 channel) path; a rolled loop here would push v[] into local memory
-                    float4* yp = reinterpret_cast<float4*>(p.y + out_off + c0);
-#pragma unroll
-                    for (int j = 0; j < 8; j++) yp[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                }
-            }
-            tc_fence_before();
-            mbar_arrive(&tempty_bar[acc]);
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == TC_MMA_WARP) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(tmem_cols));
-    }
-}
-
-// ------------------------------------------------------------------------------------------------
-// CTA-pair variant (cta_group::2) for the 256-wide layers
-//
-// One MMA instruction spans two SMs: D[256 px x 256 co]; each CTA of the pair stages its own 128 pixel rows of A
-// and HALF of the weight tile (128 of the 256 N rows), so the shared-memory -> tensor-core operand traffic per SM
-// drops from 12 KB to 8 KB per 128x256x8 step -- the binding resource of the single-CTA kernel (ncu:
-// sm__mem_tensor_cycles_active 72 %).  The leader CTA (cluster rank 0) issues the MMAs; both CTAs issue TMA into
-// their own shared memory but signal the leader's "full" barrier; tcgen05.commit multicasts "stage free" /
-// "accumulator ready" to both CTAs; both epilogues arrive on the leader's "accumulator drained" barrier.
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of `local` in the leader CTA (rank 0) of the pair
-__device__ __forceinline__ uint32_t leader_addr(uint32_t local) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local), "r"(0));
-    return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    // default semantics (release at CTA scope): the .release.cluster form costs a MEMBAR.ALL.GPU per arrival
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void tma2_load_2d(const CUtensorMap* map, uint32_t bar_cluster, void* dst, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-            smem_u32(dst)),
-        "l"(map), "r"(bar_cluster), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void tma2_load_im2col_4d(const CUtensorMap* map, uint32_t bar_cluster, void* dst, int c, int w, int h, int n,
-                                                    uint16_t off_w, uint16_t off_h) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.im2col.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2], "
-        "{%7, %8};" ::"r"(smem_u32(dst)),
-        "l"(map), "r"(bar_cluster), "r"(c), "r"(w), "r"(h), "r"(n), "h"(off_w), "h"(off_h)
-        : "memory");
-}
-__device__ __forceinline__ void umma2_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, {%5, %5, %5, %5, %5, %5, %5, %5}, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(0)
-        : "memory");
-}
-__device__ __forceinline__ void umma2_commit_mc(uint64_t* bar) {  // arrive on `bar` in BOTH CTAs of the pair
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)),
-                 "h"((uint16_t)3)
-                 : "memory");
-}
-
-constexpr int TC2_MAX_STAGES = 12;
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(TC_THREADS, 1) conv_tc2_kernel(const __grid_constant__ TcParams p) {
-    pdl_trigger();
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    constexpr int BK = TC_BK;
-    constexpr int a_bytes = TC_BM * BK * 4;      // 16 KB: one K chunk of this CTA's 128 pixel rows
-    const int b_bytes = (p.bn / 2) * BK * 4;     // 4 / 8 / 16 KB: one K chunk of this CTA's half of the bn weight rows
-    const int stage_bytes = p.cps * (a_bytes + b_bytes);  // [A_0..A_cps-1][B_0..B_cps-1]
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * stage_bytes);
-    uint64_t* empty_bar = full_bar + p.stages;
-    uint64_t* tfull_bar = empty_bar + p.stages;
-    uint64_t* tempty_bar = tfull_bar + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-    float* stat_smem = reinterpret_cast<float*>(tmem_slot + 4);  // 4 x (32 x 36) floats, only carved when p.stats
-    float4* store_patch = reinterpret_cast<float4*>(stat_smem + (p.stats ? 4 * 32 * 36 : 0));  // 4 x 2 KB, only carved when p.coalesce
-
-    const int pq = p.P * p.Q;
-    const int PT = (p.B * pq + 2 * TC_BM - 1) / (2 * TC_BM);  // pair tiles (256 pixels) per (group, class)
-    const int NT = p.Cout / p.bn;
-    const int tiles = p.G * p.ncls * NT * PT;
-    const int kchunks = p.Cin / BK;
-    const int kiters = p.KH * p.KW * kchunks;
-    const int cluster_id = blockIdx.x >> 1, nclusters = gridDim.x >> 1;
-
-    if (warp == TC_PRODUCER_WARP && lane == 0) {
-        prefetch_tmap(&p.bmap);
-        for (int c = 0; c < p.ncls; c++) prefetch_tmap(&p.cls[c].amap);
-    }
-    if (warp == TC_MMA_WARP) {
-        if (lane == 0) {
-            for (int s = 0; s < p.stages; s++) {
-                mbar_init(&full_bar[s], 1);   // leader's arrive.expect_tx covers the bytes of BOTH CTAs (the peer only issues TMA)
-                mbar_init(&empty_bar[s], 1);  // multicast commit
-            }
-            for (int a = 0; a < 2; a++) {
-                mbar_init(&tfull_bar[a], 1);     // multicast commit
-                mbar_init(&tempty_bar[a], 256);  // leader: 128 epilogue threads of each CTA
-            }
-            fence_barrier_init();
-        }
-        __syncwarp();
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;");
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    pdl_wait();  // on-chip prologue done (barriers, TMEM): from here on the kernel reads what its predecessors in the stream wrote
-
-    if (warp == TC_PRODUCER_WARP) {
-        if (lane == 0) {
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int t = cluster_id; t < tiles; t += nclusters) {
-                int pt = t % PT;
-                int r = t / PT;
-                int nt = r % NT;
-                r /= NT;
-                int c = r % p.ncls;
-                int g = r / p.ncls;
-                const TcClass& cl = p.cls[c];
-                int m0 = pt * 2 * TC_BM + (int)rank * TC_BM;
-                int img = m0 / pq;
-                int rem = m0 - img * pq;
-                int pp = rem / p.Q, qq = rem - pp * p.Q;
-                int n_coord = g * p.xg_images + img;
-                int w_coord = cl.w0 + qq * p.stride;
-                int h_coord = cl.h0 + pp * p.stride;
-                int wrow = g * p.w_rows_per_group + cl.wrow_off + nt * p.bn + (int)rank * (p.bn >> 1);
-                int kh = 0, kw = 0, kc = 0;
-                for (int k0 = 0; k0 < kiters; k0 += p.cps) {
-                    const int n = kiters - k0 < p.cps ? kiters - k0 : p.cps;
-                    mbar_wait(&empty_bar[stage], phase ^ 1);
-                    uint8_t* sa = smem + (size_t)stage * stage_bytes;
-                    uint8_t* sb = sa + p.cps * a_bytes;
-                    const uint32_t full_leader = leader_addr(smem_u32(&full_bar[stage]));
-                    // both CTAs' A + half-B land on the leader's barrier; a peer box that lands before this expect_tx only drives
-                    // the transaction count negative for a moment (the phase cannot complete before the leader's arrival)
-                    if (rank == 0) mbar_expect_tx(&full_bar[stage], (uint32_t)(2 * n * (a_bytes + b_bytes)));
-                    for (int j = 0; j < n; j++) {
-                        tma2_load_im2col_4d(&cl.amap, full_leader, sa + j * a_bytes, kc * BK, w_coord, h_coord, n_coord, (uint16_t)kw,
-                                            (uint16_t)kh);
-                        tma2_load_2d(&p.bmap, full_leader, sb + j * b_bytes, (kh * p.KW + kw) * p.Cin + kc * BK, wrow);
-                        if (++kc == kchunks) { kc = 0; if (++kw == p.KW) { kw = 0; ++kh; } }
-                    }
-                    if (++stage == p.stages) { stage = 0; phase ^= 1; }
-                }
+                out_off[h] = pix * p.Cout + nt * p.n_store;
             }
         }
-    } else if (warp == TC_MMA_WARP) {
-        if (lane == 0 && rank == 0) {
-            // kind::tf32, D=F32, K-major A and B, M = 256 (both CTAs), N = bn
-            const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(p.bn >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-            const uint64_t desc_hi = make_kmajor_sw128_desc(0);
-            int stage = 0;
-            uint32_t phase = 0;
-            int acc = 0;
-            uint32_t acc_phase = 0;
-            for (int t = cluster_id; t < tiles; t += nclusters) {
-                mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * p.bn);
-                for (int k0 = 0; k0 < kiters; k0 += p.cps) {
-                    const int n = kiters - k0 < p.cps ? kiters - k0 : p.cps;
-                    mbar_wait(&full_bar[stage], phase);
-                    tc_fence_after();
-                    const uint32_t sa = smem_u32(smem + (size_t)stage * stage_bytes);
-                    const uint32_t sb = sa + p.cps * a_bytes;
-                    for (int j = 0; j < n; j++) {
-                        const uint64_t adesc = desc_hi | (uint64_t)(((sa + j * a_bytes) & 0x3FFFF) >> 4);
-                        const uint64_t bdesc = desc_hi | (uint64_t)(((sb + j * b_bytes) & 0x3FFFF) >> 4);
+        if (p.stats) {
+            // instance-norm statistics of the raw convolution output, fused here instead of a second pass over y.  Every tile lies
+            // inside one image (P*Q % 128 == 0); each warp reduces its 16 rows per column and writes one partial chunk.
+            const int tiles_per_img = pq / TC_BM;
+            const int img = (mt * TC_BM) / pq;
+            const int chunk = ((c * tiles_per_img + (mt - img * tiles_per_img)) << 3) + cw * 4 + warp4;
+            const long col0 = (long)(g * p.B + img) * p.Cout + nt * BN + cq;
 #pragma unroll
-                        for (int kk = 0; kk < BK / 8; kk++)
-                            umma2_tf32(d_tmem, adesc + (uint64_t)(kk * 2), bdesc + (uint64_t)(kk * 2), idesc, (k0 | j | kk) != 0 ? 1u : 0u);
-                    }
-                    umma2_commit_mc(&empty_bar[stage]);
-                    if (++stage == p.stages) { stage = 0; phase ^= 1; }
+            for (int j = 0; j < BN / 8; j++) {
+                float s0 = acc[4 * j] + acc[4 * j + 2], s1 = acc[4 * j + 1] + acc[4 * j + 3];
+                float q0 = acc[4 * j] * acc[4 * j] + acc[4 * j + 2] * acc[4 * j + 2];
+                float q1 = acc[4 * j + 1] * acc[4 * j + 1] + acc[4 * j + 3] * acc[4 * j + 3];
+#pragma unroll
+                for (int o = 4; o < 32; o <<= 1) {
+                    s0 += __shfl_xor_sync(0xffffffffu, s0, o);
+                    s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+                    q0 += __shfl_xor_sync(0xffffffffu, q0, o);
+                    q1 += __shfl_xor_sync(0xffffffffu, q1, o);
                 }
-                umma2_commit_mc(&tfull_bar[acc]);
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+                if (lane < 4) *reinterpret_cast<float4*>(p.stats + ((long)chunk * p.stats_gbc + col0 + 8 * j) * 2) = make_float4(s0, q0, s1, q1);
             }
         }
-    } else {
-        const int quad = warp & 3;
-        const int row = quad * 32 + lane;
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        for (int t = cluster_id; t < tiles; t += nclusters) {
-            int pt = t % PT;
-            int r = t / PT;
-            int nt = r % NT;
-            r /= NT;
-            int c = r % p.ncls;
-            int g = r / p.ncls;
-            const TcClass& cl = p.cls[c];
-            mbar_wait(&tfull_bar[acc], acc_phase);
-            tc_fence_after();
-            const int m = pt * 2 * TC_BM + (int)rank * TC_BM + row;
-            bool valid = m < p.B * pq;
-            long out_off = 0;
-            if (valid) {
-                int img = m / pq;
-                int rem = m - img * pq;
-                int pp = rem / p.Q, qq = rem - pp * p.Q;
-                long pix = ((long)(g * p.B + img) * p.out_H + (pp * p.out_sh + cl.out_h0)) * p.out_W + (qq * p.out_sw + cl.out_w0);
-                out_off = pix * p.Cout + nt * p.bn;
-            }
-            const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * p.bn);
-            for (int c0 = 0; c0 < p.bn; c0 += 32) {
-                float v[32];
-                tmem_ld32(taddr + (uint32_t)c0, v);
-                if (p.stats) {
-                    // instance-norm statistics of the raw output in the epilogue (Conv2d -> InstanceNorm2d / AdaIN, networks.py:516-518):
-                    // this CTA's 128 rows are one 128-pixel tile inside one image (P*Q % 256 == 0); same scheme as conv_tc_kernel.
-                    // On the wide layers served by this kernel the main loop of the next tile (tens of thousands of cycles) hides it.
-                    float* patch = stat_smem + quad * (32 * 36);
-                    __syncwarp();
+        // each row's 8-column group is written by four consecutive lanes: 32 contiguous bytes, one full sector
 #pragma unroll
-                    for (int j = 0; j < 8; j++)
-                        *reinterpret_cast<float4*>(patch + lane * 36 + 4 * j) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                    __syncwarp();
-                    float cs = 0.f, cq = 0.f;
+        for (int j = 0; j < BN / 8; j++) {
+            const int col = 8 * j + cq;
+            if (col >= p.n_store) break;
+            float2 bv = make_float2(0.f, 0.f);
+            if (p.bias) bv = __ldg(reinterpret_cast<const float2*>(p.bias + (long)g * p.Cout + nt * p.n_store + col));
 #pragma unroll
-                    for (int r2 = 0; r2 < 32; r2++) {
-                        float e = patch[r2 * 36 + lane];
-                        cs += e;
-                        cq = fmaf(e, e, cq);
-                    }
-                    const int tiles_per_img = pq / TC_BM;
-                    const int mt = pt * 2 + (int)rank;
-                    const int img = (mt * TC_BM) / pq;
-                    const int chunk = ((c * tiles_per_img + (mt - img * tiles_per_img)) << 2) + quad;
-                    const long col = (long)(g * p.B + img) * p.Cout + nt * p.bn + c0 + lane;
-                    if (mt * TC_BM < p.B * pq) *reinterpret_cast<float2*>(p.stats + ((long)chunk * p.stats_gbc + col) * 2) = make_float2(cs, cq);
+            for (int h = 0; h < 2; h++) {
+                if (!valid[h]) continue;
+                float2 o = make_float2(acc[4 * j + 2 * h] + bv.x, acc[4 * j + 2 * h + 1] + bv.y);
+                if (p.addend) {
+                    const float2 a = __ldg(reinterpret_cast<const float2*>(p.addend + out_off[h] + col));
+                    o.x += a.x; o.y += a.y;
                 }
-                if (p.coalesce) {
-                    if (p.bias) {
-                        const float4* bp = reinterpret_cast<const float4*>(p.bias + (long)g * p.Cout + nt * p.bn + c0);
-#pragma unroll
-                        for (int j = 0; j < 8; j++) {
-                            float4 a = __ldg(bp + j);
-                            v[4 * j] += a.x; v[4 * j + 1] += a.y; v[4 * j + 2] += a.z; v[4 * j + 3] += a.w;
-                        }
-                    }
-                    epilogue_store_coalesced(v, store_patch + quad * 128, lane, valid ? out_off + c0 : -1, p.y, p.addend, p.mask_src, p.act, p.slope);
-                } else
-                if (valid) {
-                    if (p.bias) {
-                        const float4* bp = reinterpret_cast<const float4*>(p.bias + (long)g * p.Cout + nt * p.bn + c0);
-#pragma unroll
-                        for (int j = 0; j < 8; j++) {
-                            float4 a = __ldg(bp + j);
-                            v[4 * j] += a.x; v[4 * j + 1] += a.y; v[4 * j + 2] += a.z; v[4 * j + 3] += a.w;
-                        }
-                    }
-                    if (p.addend) {
-                        const float4* ap = reinterpret_cast<const float4*>(p.addend + out_off + c0);
-#pragma unroll
-                        for (int j = 0; j < 8; j++) {
-                            float4 a = __ldg(ap + j);
-                            v[4 * j] += a.x; v[4 * j + 1] += a.y; v[4 * j + 2] += a.z; v[4 * j + 3] += a.w;
-                        }
-                    }
-                    if (p.mask_src) {
-                        const float4* mp = reinterpret_cast<const float4*>(p.mask_src + out_off + c0);
-#pragma unroll
-                        for (int j = 0; j < 8; j++) {
-                            float4 a = __ldg(mp + j);
-                            v[4 * j] *= a.x > 0.f ? 1.f : p.slope; v[4 * j + 1] *= a.y > 0.f ? 1.f : p.slope;
-                            v[4 * j + 2] *= a.z > 0.f ? 1.f : p.slope; v[4 * j + 3] *= a.w > 0.f ? 1.f : p.slope;
-                        }
-                    } else if (p.act == CG_ACT_RELU) {
-#pragma unroll
-                        for (int j = 0; j < 32; j++) v[j] = fmaxf(v[j], 0.f);
-                    } else if (p.act == CG_ACT_LRELU) {
-#pragma unroll
-                        for (int j = 0; j < 32; j++) v[j] = v[j] > 0.f ? v[j] : v[j] * p.slope;
-                    }
-                    float4* yp = reinterpret_cast<float4*>(p.y + out_off + c0);
-#pragma unroll
-                    for (int j = 0; j < 8; j++) yp[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+                if (p.mask_src) {
+                    const float2 a = __ldg(reinterpret_cast<const float2*>(p.mask_src + out_off[h] + col));
+                    o.x *= a.x > 0.f ? 1.f : p.slope; o.y *= a.y > 0.f ? 1.f : p.slope;
+                } else if (p.act != CG_ACT_NONE) {
+                    o.x = apply_act(o.x, p.act, p.slope); o.y = apply_act(o.y, p.act, p.slope);
                 }
+                *reinterpret_cast<float2*>(p.y + out_off[h] + col) = o;
             }
-            tc_fence_before();
-            mbar_arrive_cluster(leader_addr(smem_u32(&tempty_bar[acc])));
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    if (warp == TC_MMA_WARP) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
     }
 }
+
 
 // ------------------------------------------------------------------------------------------------
 // host side
@@ -836,9 +366,6 @@ static int encode_weights_map(CUtensorMap* map, const float* w, long rows, long 
 }
 
 static int encode_weights_map_p(TcParams& p, const float* w, long rows, long ktot) {
-    p.w_base = w;
-    p.w_rows = rows;
-    p.w_ktot = ktot;
     return encode_weights_map(&p.bmap, w, rows, ktot, p.bn, p.bk);
 }
 
@@ -889,7 +416,7 @@ static int pick_bk(int cin) {
 
 // Few-tile launches (small maps: the 32x32 bottleneck of the 128x128 configuration is 8 pixel tiles per member): narrower N tiles put more
 // SMs to work.  Every extra N tile re-reads the same activation tile, from L2, which is cheap at these sizes; a 3x3 256->256 layer on
-// 1024 pixels x 2 members goes from 8 CTA pairs running 288 K-steps of 256-wide MMAs to 64 CTAs running the same steps 64 wide.
+// 1024 pixels x 2 members goes from 16 CTAs running 288 K-steps of 256-wide MMAs to 64 CTAs running the same steps 64 wide.
 static int fill_bn(int bn, long mpix, int groups_classes, int cout) {
     if (!g_small_bn) return bn;
     const int sms = sm_count_now();
@@ -908,92 +435,58 @@ bool tc_fwd_supported(const cg_conv_geom& g) {
     return true;
 }
 
+template <int BK>
+static void (*tc_kernel_for(int bn))(TcParams) {
+    switch (bn) {
+        case 16: return conv_tc_kernel<BK, 16>;
+        case 64: return conv_tc_kernel<BK, 64>;
+        case 128: return conv_tc_kernel<BK, 128>;
+        case 256: return conv_tc_kernel<BK, 256>;
+    }
+    return nullptr;
+}
+
 static int launch_tc(TcParams& p, cudaStream_t st) {
     int a_bytes = TC_BM * p.bk * 4, b_bytes = ((p.bn * p.bk * 4) + 1023) & ~1023;
     int chunk_bytes = a_bytes + b_bytes;
-    // several K chunks per stage when a chunk carries little tensor work (N <= 64 or 32-byte rows): the single MMA-issuing
-    // thread pays ~300 cycles of barrier / descriptor latency per stage
+    // several K chunks per stage when a chunk carries little tensor work (N <= 128 or 32-byte rows): fewer barrier round trips
     int kiters = p.KH * p.KW * ((p.Cin + p.bk - 1) / p.bk);
-    int cps = p.bn <= 128 ? 2 : 1;   // 48 KB (N=64) / 64 KB (N=128) stages, 4 / 3 deep
+    int cps = p.bn <= 128 ? 2 : 1;
     if (p.bk == 8) cps = 8;          // 6 KB chunks
     while (cps > 1 && (cps > kiters || cps * chunk_bytes > 64 * 1024)) cps >>= 1;
     p.cps = cps;
     int stage_bytes = cps * chunk_bytes;
-    // narrow tiles (<= 64 output channels) are the store-heavy ones; on the wide compute-bound tiles the patch traffic competes with the
-    // MMA operand reads for shared-memory bandwidth and measured 1-3 % slower (visit I): those keep the accumulator-layout stores
-    p.coalesce = g_epi_coalesce && p.bn >= 32 && (p.bn <= 64 || g_epi_coalesce == 2) && p.act != CG_ACT_TANH ? 1 : 0;
-    const int stat_bytes = (p.stats ? 4 * 32 * 36 * 4 : 0) + (p.coalesce ? 4 * 2048 : 0);
-    // narrow tiles are bound by the single MMA-issuing thread's per-stage latency: two co-resident CTAs per SM interleave their MMAs
-    const bool two = g_fwd_2cta && p.bn <= 64 && !p.stats && 2 * stage_bytes <= 100 * 1024;
-    int stages = ((two ? 112 : 226) * 1024 - 1024 - 512 - stat_bytes) / stage_bytes;  // two co-resident CTAs: 2 x (112 KB + 1 KB reserved) <= 228 KB  // 227 KB dynamic shared memory per SM
-    if (stages > 12) stages = 12;
+    int stages = (226 * 1024 - 1024 - 2 * TC_MAX_STAGES * 8) / stage_bytes;  // 227 KB dynamic shared memory per block
+    if (stages > TC_MAX_STAGES) stages = TC_MAX_STAGES;
     if (stages > 4 && stage_bytes >= 48 * 1024) stages = 4;
     if (p.n_store == 0) p.n_store = p.bn;
     p.stages = stages;
-    size_t smem = (size_t)stages * stage_bytes + 1024 /*align slack*/ + (2 * stages + 4) * 8 + 32 + stat_bytes;
+    size_t smem = (size_t)stages * stage_bytes + 1024 /*align slack*/ + 2 * stages * 8;
+    void (*kern)(TcParams) = p.bk == 32 ? tc_kernel_for<32>(p.bn) : tc_kernel_for<8>(p.bn);
+    if (!kern) {
+        set_error("conv_tc: no kernel for N tile %d / K chunk %d", p.bn, p.bk);
+        return CG_ERR_ARG;
+    }
     static PerDeviceOnce attr_set;
     if (attr_set.first()) {
-        cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        if (e != cudaSuccess) {
-            set_error("cudaFuncSetAttribute(conv_tc_kernel): %s", cudaGetErrorString(e));
-            return CG_ERR_CUDA;
+        for (int bn : {16, 64, 128, 256}) {
+            cudaError_t e = cudaFuncSetAttribute(tc_kernel_for<32>(bn), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+            if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_kernel_for<8>(bn), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+            if (e != cudaSuccess) {
+                attr_set.reset();
+                set_error("cudaFuncSetAttribute(conv_tc_kernel): %s", cudaGetErrorString(e));
+                return CG_ERR_CUDA;
+            }
         }
     }
     int MT = cdiv((long)p.B * p.P * p.Q, TC_BM);
     long tiles = (long)p.G * p.ncls * ((p.Cout + p.bn - 1) / p.bn) * MT;
-    // CTA pairs (cta_group::2): one MMA spans two SMs, each staging its own 128 pixel rows and HALF of the weight rows -> less
-    // shared-memory operand traffic per SM (wide layers) and half the MMA instructions per pixel (narrow layers, issue-bound)
-    if (((p.bn == 256 && (g_pair_mode & 1)) || (p.bn == 128 && (g_pair_mode & 2)) || (p.bn == 64 && (g_pair_mode & 4))) && p.bk == 32 && p.Cout % p.bn == 0 && p.Cin % 32 == 0 &&
-        (!p.stats || (p.P * p.Q) % (2 * TC_BM) == 0) && p.act != CG_ACT_TANH && (long)p.B * p.P * p.Q >= 512) {
-        static PerDeviceOnce attr2_set;
-        if (attr2_set.first()) {
-            cudaError_t e = cudaFuncSetAttribute(conv_tc2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-            if (e != cudaSuccess) {
-                set_error("cudaFuncSetAttribute(conv_tc2_kernel): %s", cudaGetErrorString(e));
-                return CG_ERR_CUDA;
-            }
-        }
-        const int stage2 = p.cps * (TC_BM * TC_BK * 4 + (p.bn / 2) * TC_BK * 4);
-        int stages2 = (226 * 1024 - 1536 - stat_bytes) / stage2;
-        if (stages2 > TC2_MAX_STAGES) stages2 = TC2_MAX_STAGES;
-        p.stages = stages2;
-        size_t smem2 = (size_t)stages2 * stage2 + 1024 + (2 * TC2_MAX_STAGES + 4) * 8 + 32 + stat_bytes;
-        static int max_pairs_dev[CG_MAX_DEVICES] = {0};  // co-resident CTA pairs (GPCs with an odd SM count strand one SM each)
-        int& max_pairs = max_pairs_dev[current_device()];
-        if (!max_pairs) {
-            cudaLaunchConfig_t cfg = {};
-            cfg.gridDim = dim3(2 * (sm_count_now() / 2));
-            cfg.blockDim = dim3(TC_THREADS);
-            cfg.dynamicSmemBytes = 220 * 1024;
-            cudaLaunchAttribute at;
-            at.id = cudaLaunchAttributeClusterDimension;
-            at.val.clusterDim.x = 2;
-            at.val.clusterDim.y = 1;
-            at.val.clusterDim.z = 1;
-            cfg.attrs = &at;
-            cfg.numAttrs = 1;
-            int n = 0;
-            cudaError_t e = cudaOccupancyMaxActiveClusters(&n, conv_tc2_kernel, &cfg);
-            if (e != cudaSuccess || n < 1) {
-                (void)cudaGetLastError();
-                n = sm_count_now() / 2 - 4;
-            }
-            max_pairs = n < sm_count_now() / 2 ? n : sm_count_now() / 2;
-        }
-        int pairs = g_pair_cap > 0 && g_pair_cap < max_pairs ? g_pair_cap : max_pairs;
-        if (int rc = encode_weights_map(&p.bmap, p.w_base, p.w_rows, p.w_ktot, p.bn / 2, 32)) return rc;  // each CTA stages half of the rows
-        long ptiles = (long)p.G * p.ncls * (p.Cout / p.bn) * cdiv((long)p.B * p.P * p.Q, 2 * TC_BM);
-        int nclusters = (int)(ptiles < pairs ? ptiles : pairs);
-        launch_k(conv_tc2_kernel, 2 * nclusters, TC_THREADS, smem2, st, p);
-        return check_launch("conv_tc2_kernel");
-    }
-    const long slots = (long)sm_count_now() * (two ? 2 : 1);
+    const long slots = sm_count_now();
     int grid = (int)(tiles < slots ? tiles : slots);
-    if (p.bk == 32) launch_k(conv_tc_kernel<32>, grid, TC_THREADS, smem, st, p);
-    else launch_k(conv_tc_kernel<8>, grid, TC_THREADS, smem, st, p);
+    launch_k(kern, grid, TC_THREADS, smem, st, p);
     return check_launch("conv_tc_kernel");
 }
+
 
 // nearest-upsample x2 followed by a 3x3 pad-1 convolution == four 2x2 convolutions on the ORIGINAL tensor, one per
 // output parity (a,b): output row 2i+a reads source rows {i-1,i} (a=0) or {i,i+1} (a=1), and the 3 filter rows
@@ -1031,7 +524,7 @@ int tc_fwd_stats_chunks(const cg_conv_geom& g) {
     if (pick_bn(g.Cout) < 32) return 0;
     long pq = g.ups ? (long)g.H * g.W : (long)g.Ho * g.Wo;
     if (pq % TC_BM != 0) return 0;
-    return (int)((g.ups ? 4 : 1) * (pq / TC_BM) * 4);
+    return (int)((g.ups ? 4 : 1) * (pq / TC_BM) * 8);  // one chunk per consumer warp and tile
 }
 
 int tc_conv_fwd(const cg_conv_geom& g, const float* x, const float* w, const float* bias, float* y, int act, float slope, void* ws,
@@ -1096,7 +589,7 @@ int tc_conv_fwd(const cg_conv_geom& g, const float* x, const float* w, const flo
 // so each class is a forward convolution of dy with transposed+flipped weights wt[g][class][ci][r][s][co],
 // an im2col box with lower corner -padl, and an output written with stride s at offset ihf.
 // ------------------------------------------------------------------------------------------------
-// CinP >= Cin: rows ci >= Cin are zero (pads the 8 image lanes to the minimum UMMA N of 16)
+// CinP >= Cin: rows ci >= Cin are zero (pads the 8 image lanes to the 16-wide N tile of the narrow kernels)
 // 32 (co) x 32 (ci) tiles through shared memory: reads run along ci (contiguous in OHWI), writes along co (contiguous in the
 // transposed copy); grid = (co tiles x ci tiles, KH*KW, G)
 __global__ void __launch_bounds__(256) dgrad_weight_transform_kernel(const float* __restrict__ w, float* __restrict__ wt, int Cout, int Cin,
@@ -1206,570 +699,135 @@ int tc_conv_dgrad(const cg_conv_geom& g, const float* dy, const float* w, float*
 //
 //   dW[g][co][kh][kw][ci] = sum over pixels m of dy[g][m][co] * x[g][n][p*s-pad+kh][q*s-pad+kw][ci]
 //
-// GEMM per (group, 128-cout tile, filter tap, ci tile):  D[128 co][bn ci] += A^T[pixels][co] * B[pixels][ci]
-// with the reduction (K) dimension = pixels.  Both operands are "MN-major" in shared memory: the 32-channel
-// x KP-pixel boxes TMA delivers from the channels-last tensors (dy as a plain 2-D matrix, x through the same
-// im2col map as the forward pass, at the tap's offsets, with the 32-byte-atom 128-byte swizzle) ARE the canonical
-// MN-major TF32 layout (cute::UMMA Layout_MN_SW128_32B: 32 contiguous MN elements per row, 4 K rows per 512-byte
-// atom), so no transposition is ever materialised.  The pixel range is split across CTAs (split-K) and reduced in a fixed
-// order by reduce_splits_kernel, keeping the result deterministic.
+// GEMM per (group, BM-cout tile, filter tap, BN-ci tile, pixel split):  D[BM co][BN ci] += dy^T[co][pixels] * x[pixels][ci],
+// the reduction (K) dimension being pixels.  In the channels-last tensors both operands are contiguous along their M / N
+// dimension (MN-major), and wgmma takes TF32 operands K-major only, so every 32-pixel chunk goes through a transform stage:
+// all threads load it from global memory (coalesced float4 along the channels, zero outside the image and past the split) into
+// registers and store it transposed and TF32-rounded into the K-major 128-byte-swizzled layout the forward kernel's TMA
+// produces.  Each warpgroup then multiplies 64 output channels of the chunk by the whole BN tile with wgmma.  Two shared-memory
+// buffers: the global loads and the transposed stores of chunk c+1 overlap the MMAs of chunk c.  Splits of the pixel range
+// write partial results that a second kernel sums in a fixed order (deterministic).
 // ------------------------------------------------------------------------------------------------
-constexpr int WG_KP = 32;      // pixel granularity (tensor-map box rows are kp = 32 or 64)
-constexpr int WG_NCOLS = 256;  // accumulator columns per TMEM stage = taps-per-unit * bn
+constexpr int WG_BK = 32;       // pixels per chunk = one 128-byte K-major row
 
 struct WgParams {
-    CUtensorMap amap;  // dy  [G*Mpix][Cout]  2-D, box 32 x KP
-    CUtensorMap bmap;  // x   im2col, box 32 channels x KP pixels
-    int G, xg_images, B, P, Q, Cin, Cout, KH, KW, stride, pad, bn, splits, stages;
-    int kp;            // pixels per pipeline stage: 64 when the pixel count allows (fewer, larger TMA boxes), else 32
-    int T;             // filter taps accumulated per work unit (they share the dy tile): T * bn <= 256
-    int nacc;          // TMEM accumulator stages: 2 (one CTA per SM) or 1 (two co-resident CTAs per SM share the 512 columns)
-    int Tm;            // (x-on-M variant) 128-row tiles of (tap, 32-channel block) rows per work unit: Tm * Cout <= 256
-    long Mpix, chunk;  // pixels per group; pixels per split (multiple of WG_KP)
-    float* out;        // [splits][G][Cout][KH*KW][Cin]
+    const float* x; const float* dy; float* out;
+    int G, xg_images, B, H, W, Ho, Wo, Cin, Cout, KH, KW, stride, pad;
+    long Mpix, chunk;
+    int ci_tiles;
 };
 
-// MN-major TF32 operands admit exactly one shared-memory layout (cutlass sm100_common.inl:92 "for mn-major tf32
-// operands, SW128_32B is the only available smem layout"): rows of 32 contiguous MN elements (128 B), swizzle atom =
-// 4 K-rows x 128 B with 32-byte chunks XOR-ed by the row index (Swizzle<2,5,2>) = TMA CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B,
-// descriptor layout type SWIZZLE_128B_BASE32B (1).  LBO = stride between 32-element MN groups, SBO = stride
-// between 4-row K groups (512 B); one K=8 MMA consumes two K groups.
+__device__ __forceinline__ float f4_at(const float4& v, int j) { return j == 0 ? v.x : j == 1 ? v.y : j == 2 ? v.z : v.w; }
 
-__global__ void __launch_bounds__(TC_THREADS, 2) wgrad_tc_kernel(const __grid_constant__ WgParams p) {
-    pdl_trigger();
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int box_bytes = p.kp * 128;
-    const int a_bytes = 4 * box_bytes;
-    const int nb = p.bn / 32;                     // 32-channel boxes per tap
-    const int b_bytes = (WG_NCOLS / 32) * box_bytes;
-    const int stage_bytes = a_bytes + b_bytes;
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * stage_bytes);
-    uint64_t* empty_bar = full_bar + p.stages;
-    uint64_t* tfull_bar = empty_bar + p.stages;
-    uint64_t* tempty_bar = tfull_bar + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-
-    const int taps = p.KH * p.KW;
-    const int TG = (taps + p.T - 1) / p.T;        // tap groups
-    const int COT = (p.Cout + 127) / 128;
-    const int CIT = p.Cin / p.bn;
-    const int units = p.G * COT * p.splits * CIT * TG;
-    const int tmem_cols = p.nacc * WG_NCOLS;
-
-    if (warp == TC_PRODUCER_WARP && lane == 0) {
-        prefetch_tmap(&p.amap);
-        prefetch_tmap(&p.bmap);
-    }
-    if (warp == TC_MMA_WARP) {
-        if (lane == 0) {
-            for (int s = 0; s < p.stages; s++) {
-                mbar_init(&full_bar[s], 1);
-                mbar_init(&empty_bar[s], 1);
-            }
-            for (int a = 0; a < 2; a++) {
-                mbar_init(&tfull_bar[a], 1);
-                mbar_init(&tempty_bar[a], 128);
-            }
-            fence_barrier_init();
-        }
-        __syncwarp();
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(tmem_cols));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    pdl_wait();  // on-chip prologue done (barriers, TMEM): from here on the kernel reads what its predecessors in the stream wrote
-
-    // unit -> (g, cot, split, cit, tap group), tap group fastest so CTAs running together share the dy tile in L2
-    auto decode = [&](int u, int& g, int& cot, int& sp, int& cit, int& tg) {
-        tg = u % TG; u /= TG;
-        cit = u % CIT; u /= CIT;
-        sp = u % p.splits; u /= p.splits;
-        cot = u % COT;
-        g = u / COT;
-    };
-
-    if (warp == TC_PRODUCER_WARP) {
-        // ===================== TMA producer: the whole warp issues, one box per lane =====================
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int u = blockIdx.x; u < units; u += gridDim.x) {
-            int g, cot, sp, cit, tg;
-            decode(u, g, cot, sp, cit, tg);
-            const int tap0 = tg * p.T;
-            const int tcount = taps - tap0 < p.T ? taps - tap0 : p.T;
-            const long mbeg = (long)sp * p.chunk;
-            const long mend = mbeg + p.chunk < p.Mpix ? mbeg + p.chunk : p.Mpix;
-            // lane roles: 0..3 -> dy boxes; 4..4+tcount*nb -> x boxes (tap t = q / nb, channel box j = q % nb)
-            const int q = lane - 4;
-            const bool is_a = lane < 4;
-            const bool is_b = q >= 0 && q < tcount * nb;
-            const int bt = is_b ? q / nb : 0, bj = is_b ? q - bt * nb : 0;
-            const int tap = tap0 + bt;
-            const int kh = tap / p.KW, kw = tap - kh * p.KW;
-            const uint32_t tx = (uint32_t)((4 + tcount * nb) * box_bytes);
-            for (long m = mbeg; m < mend; m += p.kp) {
-                int img = (int)(m / (p.P * p.Q));
-                int rem = (int)(m - (long)img * p.P * p.Q);
-                int pp = rem / p.Q, qq = rem - pp * p.Q;
-                mbar_wait(&empty_bar[stage], phase ^ 1);
-                uint8_t* sa = smem + (size_t)stage * stage_bytes;
-                uint8_t* sb = sa + a_bytes;
-                if (lane == 0) mbar_expect_tx(&full_bar[stage], tx);
-                __syncwarp();
-                if (is_a)
-                    tma_load_2d(&p.amap, &full_bar[stage], sa + lane * box_bytes, cot * 128 + lane * 32, (int)((long)g * p.Mpix + m));
-                if (is_b)
-                    tma_load_im2col_4d(&p.bmap, &full_bar[stage], sb + q * box_bytes, cit * p.bn + bj * 32, -p.pad + qq * p.stride,
-                                       -p.pad + pp * p.stride, g * p.xg_images + img, (uint16_t)kw, (uint16_t)kh);
-                if (++stage == p.stages) { stage = 0; phase ^= 1; }
-            }
-        }
-    } else if (warp == TC_MMA_WARP) {
-        if (lane == 0) {
-            // kind::tf32, D=F32, A and B MN-major (bits 15, 16), M=128, N=bn
-            const uint32_t idesc = make_idesc_tf32(p.bn) | (1u << 15) | (1u << 16);
-            int stage = 0;
-            uint32_t phase = 0;
-            int acc = 0;
-            uint32_t acc_phase = 0;
-            for (int u = blockIdx.x; u < units; u += gridDim.x) {
-                int g, cot, sp, cit, tg;
-                decode(u, g, cot, sp, cit, tg);
-                const int tap0 = tg * p.T;
-                const int tcount = taps - tap0 < p.T ? taps - tap0 : p.T;
-                const long mbeg = (long)sp * p.chunk;
-                const long mend = mbeg + p.chunk < p.Mpix ? mbeg + p.chunk : p.Mpix;
-                mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * WG_NCOLS);
-                uint32_t accum = 0;
-                for (long m = mbeg; m < mend; m += p.kp) {
-                    mbar_wait(&full_bar[stage], phase);
-                    tc_fence_after();
-                    uint32_t sa = smem_u32(smem + (size_t)stage * stage_bytes);
-                    uint32_t sb = sa + a_bytes;
-                    uint64_t adesc = make_mnmajor_sw128_desc(sa, box_bytes);
-                    const int nkk = p.kp / 8;
-                    for (int kk = 0; kk < nkk; kk++) {
-                        // next 8 pixels = next two 512-byte K atoms: +1024 B = +64 in the 16-byte address field
-                        for (int t = 0; t < tcount; t++) {
-                            uint64_t bdesc = make_mnmajor_sw128_desc(sb + t * nb * box_bytes, box_bytes);
-                            umma_tf32(d_tmem + (uint32_t)(t * p.bn), adesc + (uint64_t)(kk * 64), bdesc + (uint64_t)(kk * 64), idesc,
-                                      (accum | kk) ? 1u : 0u);
-                        }
-                    }
-                    accum = 1;
-                    umma_commit(&empty_bar[stage]);
-                    if (++stage == p.stages) { stage = 0; phase ^= 1; }
-                }
-                umma_commit(&tfull_bar[acc]);
-                if (++acc == p.nacc) { acc = 0; acc_phase ^= 1; }
-            }
-        }
-    } else {
-        const int quad = warp & 3;
-        const int row = quad * 32 + lane;
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        const long ktot = (long)taps * p.Cin;
-        for (int u = blockIdx.x; u < units; u += gridDim.x) {
-            int g, cot, sp, cit, tg;
-            decode(u, g, cot, sp, cit, tg);
-            const int tap0 = tg * p.T;
-            const int tcount = taps - tap0 < p.T ? taps - tap0 : p.T;
-            mbar_wait(&tfull_bar[acc], acc_phase);
-            tc_fence_after();
-            const int co = cot * 128 + row;
-            const bool valid = co < p.Cout;
-            const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * WG_NCOLS);
-            for (int t = 0; t < tcount; t++) {
-                float* op = p.out + (((long)sp * p.G + g) * p.Cout + co) * ktot + (long)(tap0 + t) * p.Cin + cit * p.bn;
-                for (int c0 = 0; c0 < p.bn; c0 += 32) {
-                    float v[32];
-                    tmem_ld32(taddr + (uint32_t)(t * p.bn + c0), v);
-                    if (valid) {
-                        float4* yp = reinterpret_cast<float4*>(op + c0);
+// rows r0..r0+3 of a K-major 128-byte-swizzled operand tile (rows of 32 fp32), column k
+__device__ __forceinline__ void store_kmajor4(uint8_t* tile, int r0, int k, const float4& v) {
 #pragma unroll
-                        for (int j = 0; j < 8; j++) yp[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                    }
-                }
-            }
-            tc_fence_before();
-            mbar_arrive(&tempty_bar[acc]);
-            if (++acc == p.nacc) { acc = 0; acc_phase ^= 1; }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == TC_MMA_WARP) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(tmem_cols));
+    for (int j = 0; j < 4; j++) {
+        const int r = r0 + j;
+        *reinterpret_cast<float*>(tile + (r >> 3) * 1024 + (r & 7) * 128 + (((k >> 2) ^ (r & 7)) << 4) + (k & 3) * 4) = to_tf32(f4_at(v, j));
     }
 }
 
-// CTA-pair variant of the weight gradient: one 256-cout x N tile per pair.  Each CTA stages dy for its own 128 output
-// channels and HALF of the x columns of every tap (N/2), so a 64-pixel stage is 64 KB instead of 96 KB (3 stages deep
-// instead of 2, 8 TMA boxes instead of 12) and the x tile crosses L2 -> shared memory once per 256 output channels.
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(TC_THREADS, 1) wgrad_tc2_kernel(const __grid_constant__ WgParams p) {
+template <int BM, int BN>
+__global__ void __launch_bounds__(2 * BM) wgrad_tc_kernel(const __grid_constant__ WgParams p) {
+    constexpr int NWARPS = 2 * BM / 32;             // BM / 64 warpgroups
+    constexpr int NA = 4, NB = 4 * BN / BM;         // float4 loads per thread and chunk: dy, x
+    constexpr int A_BYTES = BM * 128, STAGE = (BM + BN) * 128;
     pdl_trigger();
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const int box_bytes = p.kp * 128;
-    const int a_bytes = 4 * box_bytes;
-    const int nb2 = p.bn / 64;                    // 32-channel boxes per tap staged by THIS CTA (half of the tap's N)
-    const int b_bytes = (WG_NCOLS / 64) * box_bytes;
-    const int stage_bytes = a_bytes + b_bytes;
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * stage_bytes);
-    uint64_t* empty_bar = full_bar + p.stages;
-    uint64_t* tfull_bar = empty_bar + p.stages;
-    uint64_t* tempty_bar = tfull_bar + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
+    const int lane = threadIdx.x & 31;
+    const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);  // warp-uniform for the compiler
+    const int wg = warp >> 2;
+    const int tap = blockIdx.x / p.ci_tiles, ci0 = (blockIdx.x % p.ci_tiles) * BN;
+    const int kh = tap / p.KW, kw = tap - kh * p.KW;
+    const int co0 = blockIdx.y * BM;
+    const int g = blockIdx.z % p.G, split = blockIdx.z / p.G;
+    const long m_begin = (long)split * p.chunk;
+    long m_end = m_begin + p.chunk;
+    if (m_end > p.Mpix) m_end = p.Mpix;
+    const int PQ = p.Ho * p.Wo;
+    const float* dyg = p.dy + (long)g * p.Mpix * p.Cout;
+    // loader mapping: a warp covers 8 pixels x 4 float4 columns per load (full 64-byte runs in global memory, at most 2-way bank
+    // conflicts on the transposed stores); load i of warp w reads column block (w + NWARPS i) / 4 of this thread's single pixel
+    const int kq = lane & 7, cq = lane >> 3;
+    const int k_own = 8 * (warp & 3) + kq;
+    pdl_wait();
 
-    const int taps = p.KH * p.KW;
-    const int TG = (taps + p.T - 1) / p.T;
-    const int COT = p.Cout / 256;
-    const int CIT = p.Cin / p.bn;
-    const int units = p.G * COT * p.splits * CIT * TG;
-    const int cluster_id = blockIdx.x >> 1, nclusters = gridDim.x >> 1;
-
-    if (warp == TC_PRODUCER_WARP && lane == 0) {
-        prefetch_tmap(&p.amap);
-        prefetch_tmap(&p.bmap);
-    }
-    if (warp == TC_MMA_WARP) {
-        if (lane == 0) {
-            for (int s = 0; s < p.stages; s++) {
-                mbar_init(&full_bar[s], 1);
-                mbar_init(&empty_bar[s], 1);
-            }
-            for (int a = 0; a < 2; a++) {
-                mbar_init(&tfull_bar[a], 1);
-                mbar_init(&tempty_bar[a], 256);
-            }
-            fence_barrier_init();
+    float4 ra[NA], rb[NB];
+    auto gload = [&](long m0) {
+        const long m = m0 + k_own;
+        const bool in = m < m_end;
+        const float* xs = nullptr;
+        if (in) {
+            const int img = (int)(m / PQ);
+            const int rem = (int)(m - (long)img * PQ);
+            const int oh = rem / p.Wo, ow = rem - oh * p.Wo;
+            const int ih = oh * p.stride - p.pad + kh, iw = ow * p.stride - p.pad + kw;
+            if (ih >= 0 && ih < p.H && iw >= 0 && iw < p.W) xs = p.x + (((long)(g * p.xg_images + img) * p.H + ih) * p.W + iw) * p.Cin;
         }
-        __syncwarp();
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(2 * WG_NCOLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;");
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    pdl_wait();  // on-chip prologue done (barriers, TMEM): from here on the kernel reads what its predecessors in the stream wrote
-
-    auto decode = [&](int u, int& g, int& cot, int& sp, int& cit, int& tg) {
-        tg = u % TG; u /= TG;
-        cit = u % CIT; u /= CIT;
-        sp = u % p.splits; u /= p.splits;
-        cot = u % COT;
-        g = u / COT;
+#pragma unroll
+        for (int i = 0; i < NA; i++) {
+            const int co = co0 + 4 * (4 * ((warp + NWARPS * i) >> 2) + cq);
+            ra[i] = in && co < p.Cout ? __ldg(reinterpret_cast<const float4*>(dyg + m * p.Cout + co)) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+#pragma unroll
+        for (int i = 0; i < NB; i++) {
+            const int ci = ci0 + 4 * (4 * ((warp + NWARPS * i) >> 2) + cq);
+            rb[i] = xs && ci < p.Cin ? __ldg(reinterpret_cast<const float4*>(xs + ci)) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+    };
+    auto sstore = [&](int buf) {
+        uint8_t* sa = smem + buf * STAGE;
+#pragma unroll
+        for (int i = 0; i < NA; i++) store_kmajor4(sa, 4 * (4 * ((warp + NWARPS * i) >> 2) + cq), k_own, ra[i]);
+#pragma unroll
+        for (int i = 0; i < NB; i++) store_kmajor4(sa + A_BYTES, 4 * (4 * ((warp + NWARPS * i) >> 2) + cq), k_own, rb[i]);
     };
 
-    if (warp == TC_PRODUCER_WARP) {
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int u = cluster_id; u < units; u += nclusters) {
-            int g, cot, sp, cit, tg;
-            decode(u, g, cot, sp, cit, tg);
-            const int tap0 = tg * p.T;
-            const int tcount = taps - tap0 < p.T ? taps - tap0 : p.T;
-            const long mbeg = (long)sp * p.chunk;
-            const long mend = mbeg + p.chunk < p.Mpix ? mbeg + p.chunk : p.Mpix;
-            // lane roles: 0..3 -> dy boxes of this CTA's 128 couts; 4..4+tcount*nb2 -> this CTA's half of each tap's x boxes
-            const int q = lane - 4;
-            const bool is_a = lane < 4;
-            const bool is_b = q >= 0 && q < tcount * nb2;
-            const int bt = is_b ? q / nb2 : 0, bj = is_b ? q - bt * nb2 : 0;
-            const int tap = tap0 + bt;
-            const int kh = tap / p.KW, kw = tap - kh * p.KW;
-            const uint32_t tx = (uint32_t)(2 * (4 + tcount * nb2) * box_bytes);  // both CTAs' boxes land on the leader's barrier
-            for (long m = mbeg; m < mend; m += p.kp) {
-                int img = (int)(m / (p.P * p.Q));
-                int rem = (int)(m - (long)img * p.P * p.Q);
-                int pp = rem / p.Q, qq = rem - pp * p.Q;
-                mbar_wait(&empty_bar[stage], phase ^ 1);
-                uint8_t* sa = smem + (size_t)stage * stage_bytes;
-                uint8_t* sb = sa + a_bytes;
-                const uint32_t full_leader = leader_addr(smem_u32(&full_bar[stage]));
-                if (lane == 0 && rank == 0) mbar_expect_tx(&full_bar[stage], tx);
-                __syncwarp();
-                if (is_a)
-                    tma2_load_2d(&p.amap, full_leader, sa + lane * box_bytes, cot * 256 + (int)rank * 128 + lane * 32,
-                                 (int)((long)g * p.Mpix + m));
-                if (is_b)
-                    tma2_load_im2col_4d(&p.bmap, full_leader, sb + q * box_bytes, cit * p.bn + (int)rank * (p.bn >> 1) + bj * 32,
-                                        -p.pad + qq * p.stride, -p.pad + pp * p.stride, g * p.xg_images + img, (uint16_t)kw, (uint16_t)kh);
-                if (++stage == p.stages) { stage = 0; phase ^= 1; }
-            }
-        }
-    } else if (warp == TC_MMA_WARP) {
-        if (lane == 0 && rank == 0) {
-            // kind::tf32, D=F32, A and B MN-major (bits 15, 16), M = 256 (both CTAs), N = bn
-            const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(p.bn >> 3) << 17) |
-                                   ((uint32_t)(256 >> 4) << 24);
-            int stage = 0;
-            uint32_t phase = 0;
-            int acc = 0;
-            uint32_t acc_phase = 0;
-            for (int u = cluster_id; u < units; u += nclusters) {
-                int g, cot, sp, cit, tg;
-                decode(u, g, cot, sp, cit, tg);
-                const int tap0 = tg * p.T;
-                const int tcount = taps - tap0 < p.T ? taps - tap0 : p.T;
-                const long mbeg = (long)sp * p.chunk;
-                const long mend = mbeg + p.chunk < p.Mpix ? mbeg + p.chunk : p.Mpix;
-                mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * WG_NCOLS);
-                uint32_t accum = 0;
-                for (long m = mbeg; m < mend; m += p.kp) {
-                    mbar_wait(&full_bar[stage], phase);
-                    tc_fence_after();
-                    uint32_t sa = smem_u32(smem + (size_t)stage * stage_bytes);
-                    uint32_t sb = sa + a_bytes;
-                    uint64_t adesc = make_mnmajor_sw128_desc(sa, box_bytes);
-                    const int nkk = p.kp / 8;
-                    for (int kk = 0; kk < nkk; kk++) {
-                        for (int t = 0; t < tcount; t++) {
-                            uint64_t bdesc = make_mnmajor_sw128_desc(sb + t * nb2 * box_bytes, box_bytes);
-                            umma2_tf32(d_tmem + (uint32_t)(t * p.bn), adesc + (uint64_t)(kk * 64), bdesc + (uint64_t)(kk * 64), idesc,
-                                       (accum | kk) ? 1u : 0u);
-                        }
-                    }
-                    accum = 1;
-                    umma2_commit_mc(&empty_bar[stage]);
-                    if (++stage == p.stages) { stage = 0; phase ^= 1; }
-                }
-                umma2_commit_mc(&tfull_bar[acc]);
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-            }
-        }
-    } else {
-        const int quad = warp & 3;
-        const int row = quad * 32 + lane;
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        const long ktot = (long)taps * p.Cin;
-        for (int u = cluster_id; u < units; u += nclusters) {
-            int g, cot, sp, cit, tg;
-            decode(u, g, cot, sp, cit, tg);
-            const int tap0 = tg * p.T;
-            const int tcount = taps - tap0 < p.T ? taps - tap0 : p.T;
-            mbar_wait(&tfull_bar[acc], acc_phase);
-            tc_fence_after();
-            const int co = cot * 256 + (int)rank * 128 + row;
-            const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * WG_NCOLS);
-            for (int t = 0; t < tcount; t++) {
-                float* op = p.out + (((long)sp * p.G + g) * p.Cout + co) * ktot + (long)(tap0 + t) * p.Cin + cit * p.bn;
-                for (int c0 = 0; c0 < p.bn; c0 += 32) {
-                    float v[32];
-                    tmem_ld32(taddr + (uint32_t)(t * p.bn + c0), v);
-                    float4* yp = reinterpret_cast<float4*>(op + c0);
+    const uint64_t desc0 = make_kmajor_sw128_desc(0);
+    const long nchunks = (m_end - m_begin + WG_BK - 1) / WG_BK;
+    float acc[BN / 2];
+    gload(m_begin);
+    sstore(0);
+    fence_proxy_async();
+    __syncthreads();
+    for (long c = 0; c < nchunks; c++) {
+        const int buf = (int)(c & 1);
+        if (c + 1 < nchunks) gload(m_begin + (c + 1) * WG_BK);
+        const uint32_t sa = smem_u32(smem + buf * STAGE) + wg * (64 * 128);
+        const uint32_t sb = smem_u32(smem + buf * STAGE) + A_BYTES;
+        const uint64_t adesc = desc0 | (uint64_t)((sa & 0x3FFFF) >> 4), bdesc = desc0 | (uint64_t)((sb & 0x3FFFF) >> 4);
+        wgmma_fence();
 #pragma unroll
-                    for (int j = 0; j < 8; j++) yp[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                }
-            }
-            tc_fence_before();
-            mbar_arrive_cluster(leader_addr(smem_u32(&tempty_bar[acc])));
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+        for (int kk = 0; kk < WG_BK / 8; kk++)  // 8 tf32 (32 bytes) along K per step: +2 in the address field
+            wgmma_tf32<BN>(acc, adesc + (uint64_t)(kk * 2), bdesc + (uint64_t)(kk * 2), (c | kk) != 0 ? 1 : 0);
+        wgmma_commit();
+        if (c + 1 < nchunks) {
+            wgmma_wait<1>();  // this warpgroup's MMAs of chunk c-1 have retired ...
+            __syncthreads();  // ... and the other warpgroup's: the other buffer is free
+            sstore(buf ^ 1);
+            fence_proxy_async();
+            __syncthreads();
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    if (warp == TC_MMA_WARP) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(2 * WG_NCOLS));
-    }
-}
+    wgmma_wait<0>();
+    wgmma_reg_fence(acc, BN / 2);
 
-// Weight gradient with the roles swapped, for layers with <= 64 output channels: the 128 MMA rows are four (tap, 32-channel
-// block) row groups of x instead of output channels (which would leave half of every M = 128 instruction empty), dy is the N
-// operand (N = Cout).  D[(tap, ci)][co] is written back transposed: for a fixed co the 32 lanes of a warp hold 32
-// consecutive ci = one 128-byte store.  Up to Tm row tiles share the dy stage.
-__global__ void __launch_bounds__(TC_THREADS, 2) wgrad_xm_kernel(const __grid_constant__ WgParams p) {
-    pdl_trigger();
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int box_bytes = p.kp * 128;
-    const int nbo = p.Cout / 32;                  // dy boxes (1 or 2)
-    const int a_bytes = 2 * box_bytes;            // dy slot (N operand)
-    const int b_bytes = p.Tm * 4 * box_bytes;     // x row groups (M operand)
-    const int stage_bytes = a_bytes + b_bytes;
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * stage_bytes);
-    uint64_t* empty_bar = full_bar + p.stages;
-    uint64_t* tfull_bar = empty_bar + p.stages;
-    uint64_t* tempty_bar = tfull_bar + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-
-    const int CB = p.Cin / 32;                    // 32-channel blocks per tap
-    const int RG = p.KH * p.KW * CB;              // row groups in all
-    const int GPU_ = p.Tm * 4;                    // row groups per unit
-    const int MG = (RG + GPU_ - 1) / GPU_;
-    const int units = p.G * p.splits * MG;
-    const int acc_cols = p.nacc == 1 ? WG_NCOLS / 2 : WG_NCOLS;  // nacc == 1 flags two co-resident CTAs: 2 x 128 columns each
-    const int tmem_cols = 2 * acc_cols;
-
-    if (warp == TC_PRODUCER_WARP && lane == 0) {
-        prefetch_tmap(&p.amap);
-        prefetch_tmap(&p.bmap);
-    }
-    if (warp == TC_MMA_WARP) {
-        if (lane == 0) {
-            for (int s = 0; s < p.stages; s++) {
-                mbar_init(&full_bar[s], 1);
-                mbar_init(&empty_bar[s], 1);
-            }
-            for (int a = 0; a < 2; a++) {
-                mbar_init(&tfull_bar[a], 1);
-                mbar_init(&tempty_bar[a], 128);
-            }
-            fence_barrier_init();
-        }
-        __syncwarp();
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(tmem_cols));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    pdl_wait();  // on-chip prologue done (barriers, TMEM): from here on the kernel reads what its predecessors in the stream wrote
-
-    // unit -> (g, split, row-tile group), row-tile group fastest so CTAs running together share the dy tile in L2
-    auto decode = [&](int u, int& g, int& sp, int& mg) {
-        mg = u % MG; u /= MG;
-        sp = u % p.splits;
-        g = u / p.splits;
-    };
-
-    if (warp == TC_PRODUCER_WARP) {
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int u = blockIdx.x; u < units; u += gridDim.x) {
-            int g, sp, mg;
-            decode(u, g, sp, mg);
-            const int rg0 = mg * GPU_;
-            const int ng = RG - rg0 < GPU_ ? RG - rg0 : GPU_;  // row groups of this unit
-            const long mbeg = (long)sp * p.chunk;
-            const long mend = mbeg + p.chunk < p.Mpix ? mbeg + p.chunk : p.Mpix;
-            // lane roles: 0..nbo-1 -> dy boxes; 2..2+ng -> x row groups (tap, channel block)
-            const int q = lane - 2;
-            const bool is_a = lane < nbo;
-            const bool is_b = q >= 0 && q < ng;
-            const int rg = is_b ? rg0 + q : 0;
-            const int tap = rg / CB, cb = rg - tap * CB;
-            const int kh = tap / p.KW, kw = tap - kh * p.KW;
-            const uint32_t tx = (uint32_t)((nbo + ng) * box_bytes);
-            for (long m = mbeg; m < mend; m += p.kp) {
-                int img = (int)(m / (p.P * p.Q));
-                int rem = (int)(m - (long)img * p.P * p.Q);
-                int pp = rem / p.Q, qq = rem - pp * p.Q;
-                mbar_wait(&empty_bar[stage], phase ^ 1);
-                uint8_t* sa = smem + (size_t)stage * stage_bytes;
-                uint8_t* sb = sa + a_bytes;
-                if (lane == 0) mbar_expect_tx(&full_bar[stage], tx);
-                __syncwarp();
-                if (is_a) tma_load_2d(&p.amap, &full_bar[stage], sa + lane * box_bytes, lane * 32, (int)((long)g * p.Mpix + m));
-                if (is_b)
-                    tma_load_im2col_4d(&p.bmap, &full_bar[stage], sb + q * box_bytes, cb * 32, -p.pad + qq * p.stride, -p.pad + pp * p.stride,
-                                       g * p.xg_images + img, (uint16_t)kw, (uint16_t)kh);
-                if (++stage == p.stages) { stage = 0; phase ^= 1; }
-            }
-        }
-    } else if (warp == TC_MMA_WARP) {
-        if (lane == 0) {
-            // kind::tf32, D=F32, A (x) and B (dy) MN-major (bits 15, 16), M=128, N=Cout
-            const uint32_t idesc = make_idesc_tf32(p.Cout) | (1u << 15) | (1u << 16);
-            int stage = 0;
-            uint32_t phase = 0;
-            int acc = 0;
-            uint32_t acc_phase = 0;
-            for (int u = blockIdx.x; u < units; u += gridDim.x) {
-                int g, sp, mg;
-                decode(u, g, sp, mg);
-                const int rg0 = mg * GPU_;
-                const int ng = RG - rg0 < GPU_ ? RG - rg0 : GPU_;
-                const int ntile = (ng + 3) >> 2;
-                const long mbeg = (long)sp * p.chunk;
-                const long mend = mbeg + p.chunk < p.Mpix ? mbeg + p.chunk : p.Mpix;
-                mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * acc_cols);
-                uint32_t accum = 0;
-                for (long m = mbeg; m < mend; m += p.kp) {
-                    mbar_wait(&full_bar[stage], phase);
-                    tc_fence_after();
-                    uint32_t sa = smem_u32(smem + (size_t)stage * stage_bytes);
-                    uint32_t sb = sa + a_bytes;
-                    uint64_t ndesc = make_mnmajor_sw128_desc(sa, box_bytes);  // dy: N operand
-                    const int nkk = p.kp / 8;
-                    for (int kk = 0; kk < nkk; kk++) {
-                        for (int t = 0; t < ntile; t++) {
-                            // a partial last tile multiplies stale shared memory in its missing row groups: those D rows are never stored
-                            uint64_t mdesc = make_mnmajor_sw128_desc(sb + t * 4 * box_bytes, box_bytes);
-                            umma_tf32(d_tmem + (uint32_t)(t * p.Cout), mdesc + (uint64_t)(kk * 64), ndesc + (uint64_t)(kk * 64), idesc,
-                                      (accum | kk) ? 1u : 0u);
-                        }
-                    }
-                    accum = 1;
-                    umma_commit(&empty_bar[stage]);
-                    if (++stage == p.stages) { stage = 0; phase ^= 1; }
-                }
-                umma_commit(&tfull_bar[acc]);
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-            }
-        }
-    } else {
-        const int quad = warp & 3;
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        const long ktot = (long)p.KH * p.KW * p.Cin;
-        for (int u = blockIdx.x; u < units; u += gridDim.x) {
-            int g, sp, mg;
-            decode(u, g, sp, mg);
-            const int rg0 = mg * GPU_;
-            const int ng = RG - rg0 < GPU_ ? RG - rg0 : GPU_;
-            const int ntile = (ng + 3) >> 2;
-            mbar_wait(&tfull_bar[acc], acc_phase);
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * acc_cols);
-            for (int t = 0; t < ntile; t++) {
-                const int q = t * 4 + quad;          // this warp's row group inside the unit
-                const bool valid = q < ng;
-                const int rg = rg0 + q;
-                const int tap = rg / CB, cb = rg - tap * CB;
-                // dw[sp][g][co][tap][ci], ci = cb*32 + lane: one 128-byte store per output channel
-                float* op = p.out + ((long)sp * p.G + g) * p.Cout * ktot + (long)tap * p.Cin + cb * 32 + lane;
-                for (int c0 = 0; c0 < p.Cout; c0 += 32) {
-                    float v[32];
-                    tmem_ld32(taddr + (uint32_t)(t * p.Cout + c0), v);
-                    if (valid) {
+    const long Ktot = (long)p.KH * p.KW * p.Cin;
+    float* out = p.out + (long)split * p.G * p.Cout * Ktot;
+    const int row0 = co0 + wg * 64 + 16 * (warp & 3) + (lane >> 2);
 #pragma unroll
-                        for (int j = 0; j < 32; j++) op[(long)(c0 + j) * ktot] = v[j];
-                    }
-                }
-            }
-            tc_fence_before();
-            mbar_arrive(&tempty_bar[acc]);
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+    for (int j = 0; j < BN / 8; j++) {
+        const int ci = ci0 + 8 * j + 2 * (lane & 3);
+        if (ci >= p.Cin) continue;
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const int co = row0 + 8 * h;
+            if (co < p.Cout)
+                *reinterpret_cast<float2*>(out + ((long)g * p.Cout + co) * Ktot + (long)tap * p.Cin + ci) =
+                    make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == TC_MMA_WARP) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(tmem_cols));
     }
 }
 
@@ -1786,80 +844,33 @@ __global__ void reduce_splits_tc_kernel(const float* __restrict__ part, float* _
     reinterpret_cast<float4*>(out)[i] = s;
 }
 
-static int wg_bn(int cin) {
-    if (cin % 256 == 0) return 256;
-    if (cin % 32 == 0 && cin < 256) return cin;  // 32 .. 224: one N tile
-    return 0;
-}
+// Tile shape: 128 output / input channels where the layer has more than 64, else 64
+static int wg_bm(const cg_conv_geom& g) { return g.Cout > 64 ? 128 : 64; }
+static int wg_bn(const cg_conv_geom& g) { return g.Cin > 64 ? 128 : 64; }
 
-// CTA pairs (256 output channels per unit) when the layer has them and every tap's N splits into two 32-channel-box halves
-static bool wg_pair(const cg_conv_geom& g) { return (g_pair_mode & 8) && g.Cout % 256 == 0 && wg_bn(g.Cin) % 64 == 0; }
-// x-on-M variant for <= 64 output channels (a 128-row cout tile would be half empty)
-static bool wg_xm(const cg_conv_geom& g) { return g_wgrad_xm && (g.Cout == 64 || g.Cout == 32) && g.Cin % 32 == 0; }
-static int wg_xm_tm(const cg_conv_geom& g) {
-    int rg = g.KH * g.KW * (g.Cin / 32), mt = (rg + 3) / 4;
-    int tm = WG_NCOLS / g.Cout;  // TMEM columns
-    if (tm > 2) tm = 2;          // 2 dy + 8 x boxes per 64-pixel stage = 80 KB, two stages (three tiles = 112 KB would leave one)
-    if (tm > mt) tm = mt;
-    return tm;
-}
-// 64-pixel stages (fewer, larger TMA boxes) for the one-CTA-per-SM kernels; the plain kernel runs two CTAs per SM with 32-pixel stages
-static bool wg_two(const cg_conv_geom& g) { return g_wgrad_2cta && !wg_pair(g) && (!wg_xm(g) || g_wgrad_xm2); }
-static int wg_kp(const cg_conv_geom& g) { return (!wg_two(g) && ((long)g.B * g.Ho * g.Wo) % 64 == 0) ? 64 : 32; }
+// Split the pixel range until the launch fills every SM several times over (up to 3 co-resident CTAs each), keeping >= 8 chunks
+// of work per split and the partial sums <= 64 MB.
 static void wg_plan(const cg_conv_geom& g, int& splits, long& chunk) {
-    long Mpix = (long)g.B * g.Ho * g.Wo;
-    const int kp = wg_kp(g);
-    int bn = wg_bn(g.Cin);
-    int T = WG_NCOLS / bn;
-    if (T > g.KH * g.KW) T = g.KH * g.KW;
-    const bool pair = wg_pair(g);
-    long base = (long)g.G * (pair ? g.Cout / 256 : (g.Cout + 127) / 128) * (g.Cin / bn) * ((g.KH * g.KW + T - 1) / T);
-    if (wg_xm(g)) {
-        int tm = wg_xm_tm(g);
-        int rgs = g.KH * g.KW * (g.Cin / 32);
-        base = (long)g.G * ((rgs + tm * 4 - 1) / (tm * 4));
-    }
-    init_driver();
-    const int sms = (sm_count_now() > 0 ? sm_count_now() : 148) * (wg_two(g) ? 2 : 1) / (pair ? 2 : 1);
-    long maxs = Mpix / (kp * 8);  // at least 8 pipeline stages of work per split
-    if (maxs < 1) maxs = 1;
+    const long Mpix = (long)g.B * g.Ho * g.Wo;
+    const long base = (long)g.G * cdiv(g.Cout, wg_bm(g)) * cdiv(g.Cin, wg_bn(g)) * g.KH * g.KW;
+    const long target = 3L * sm_count_now();
+    long s = (target + base - 1) / base;
+    long maxs = Mpix / (8 * WG_BK);
+    const long out_bytes = (long)g.G * g.Cout * g.KH * g.KW * g.Cin * 4;
+    const long cap = (64l << 20) / (out_bytes > 0 ? out_bytes : 1);
+    if (maxs > cap) maxs = cap;
     if (maxs > 64) maxs = 64;
-    // pick the split count whose unit count fills whole waves best (persistent grid = #SMs), preferring >= 3 waves
-    int best = 1;
-    double best_score = -1.0;
-    for (int s = 1; s <= maxs; s++) {
-        long units = base * s;
-        long waves = (units + sms - 1) / sms;
-        double eff = (double)units / (double)(waves * sms);
-        double score = eff - 0.01 * s - (waves < 3 ? 0.15 * (3 - waves) : 0.0);
-        if (score > best_score) { best_score = score; best = s; }
-    }
-    // Small problems (few output tiles, e.g. a 1x1 64->64 layer: 2 units per member): the score above never leaves one split because
-    // each extra split fills < 1 % of a wave, and two CTAs then walk all the pixels (0.15 ms for 134 MFLOP at 128x128).  Below half a
-    // wave, take as many splits as fill one wave (each still >= 8 pipeline stages), capped so the partial sums stay <= 32 MB.
-    if (g_small_bn && base * best * 2 < sms) {
-        long fill = sms / base;
-        const long out_bytes = (long)g.G * g.Cout * g.KH * g.KW * g.Cin * 4;
-        const long cap = (32l << 20) / (out_bytes > 0 ? out_bytes : 1);
-        if (fill > cap) fill = cap;
-        if (fill > maxs) fill = maxs;
-        if (fill > best) best = (int)fill;
-    }
-    splits = best;
-    chunk = ((Mpix + splits - 1) / splits + kp - 1) / kp * kp;
+    if (s > maxs) s = maxs;
+    if (s < 1) s = 1;
+    chunk = ((Mpix + s - 1) / s + WG_BK - 1) / WG_BK * WG_BK;
     splits = (int)((Mpix + chunk - 1) / chunk);
 }
 
 bool tc_wgrad_supported(const cg_conv_geom& g) {
-    init_driver();
-    if (!g_encode_tiled || !g_encode_im2col) return false;
     if (g.ups) return false;
-    if (wg_bn(g.Cin) == 0) return false;
-    if (g.Cout % 4 != 0) return false;
+    if (g.Cin % 32 != 0 || g.Cout % 4 != 0) return false;
     long Mpix = (long)g.B * g.Ho * g.Wo;
-    if (Mpix % WG_KP != 0 || Mpix < 256) return false;
-    if (g.pad > 120 || g.KH > 120) return false;
-    return true;
+    return Mpix % WG_BK == 0 && Mpix >= 256;
 }
 
 size_t tc_wgrad_ws(const cg_conv_geom& g) {
@@ -1869,182 +880,44 @@ size_t tc_wgrad_ws(const cg_conv_geom& g) {
     return (size_t)splits * g.G * g.Cout * g.KH * g.KW * g.Cin * sizeof(float);
 }
 
-// dy [rows][C] as a 2-D tensor map with 32-channel x kp-pixel boxes in the MN-major TF32 layout (also used by conv_img.cu)
-static int encode_mn_map_raw(CUtensorMap* map, const float* t, long rows, int C, int kp) {
-    init_driver();
-    if (!g_encode_tiled) {
-        set_error("cuTensorMapEncodeTiled unavailable");
-        return CG_ERR_CUDA;
-    }
-    cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)rows};
-    cuuint64_t strides[1] = {(cuuint64_t)C * 4};
-    cuuint32_t box[2] = {32, (cuuint32_t)kp};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = g_encode_tiled(map, CU_TENSOR_MAP_DATA_TYPE_TFLOAT32, 2, (void*)t, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        set_error("cuTensorMapEncodeTiled(mn-major map rows=%ld C=%d) failed: %d", rows, C, (int)r);
-        return CG_ERR_CUDA;
-    }
-    return CG_OK;
-}
-int tc_encode_mn_map(CUtensorMap* map, const float* t, long rows, int C, int kp) {
-    MapKey k{};
-    k.ptr = t; k.a = rows; k.v[0] = C; k.v[1] = kp; k.v[7] = 3;
-    return cached_map(map, k, [&](CUtensorMap* m) { return encode_mn_map_raw(m, t, rows, C, kp); });
-}
-// y [rows][C] fp32 as a 2-D store map with 32-channel x box_rows boxes, 128-byte swizzled shared-memory side (epilogues that stage
-// their tile in shared memory and leave through cp.async.bulk.tensor stores)
-static int encode_store_map_raw(CUtensorMap* map, float* t, long rows, int C, int box_rows) {
-    init_driver();
-    if (!g_encode_tiled) {
-        set_error("cuTensorMapEncodeTiled unavailable");
-        return CG_ERR_CUDA;
-    }
-    cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)rows};
-    cuuint64_t strides[1] = {(cuuint64_t)C * 4};
-    cuuint32_t box[2] = {32, (cuuint32_t)box_rows};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = g_encode_tiled(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)t, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        set_error("cuTensorMapEncodeTiled(store map rows=%ld C=%d) failed: %d", rows, C, (int)r);
-        return CG_ERR_CUDA;
-    }
-    return CG_OK;
-}
-int tc_encode_store_map(CUtensorMap* map, float* t, long rows, int C, int box_rows) {
-    MapKey k{};
-    k.ptr = t; k.a = rows; k.v[0] = C; k.v[1] = box_rows; k.v[7] = 4;
-    return cached_map(map, k, [&](CUtensorMap* m) { return encode_store_map_raw(m, t, rows, C, box_rows); });
-}
 int tc_sm_count() { return sm_count_now(); }
 
 int tc_conv_wgrad(const cg_conv_geom& g, const float* x, const float* dy, float* dw, void* ws, size_t ws_bytes, cudaStream_t st) {
-    init_driver();
     WgParams p{};
-    wg_plan(g, p.splits, p.chunk);
+    int splits;
+    wg_plan(g, splits, p.chunk);
     size_t need = tc_wgrad_ws(g);
     if (need > ws_bytes) {
         set_error("conv_wgrad(tc): workspace %zu < %zu bytes", ws_bytes, need);
         return CG_ERR_WORKSPACE;
     }
-    p.bn = wg_bn(g.Cin);
-    p.kp = wg_kp(g);
-    p.Mpix = (long)g.B * g.Ho * g.Wo;
-    if (int rc = tc_encode_mn_map(&p.amap, dy, (long)g.G * p.Mpix, g.Cout, p.kp)) return rc;
-    long nimg = (long)(g.x_groups == 1 ? 1 : g.G) * g.B;
-    {
-        MapKey k{};
-        k.ptr = x; k.a = nimg; k.b = ((int64_t)g.H << 32) | (uint32_t)g.W;
-        k.v[0] = g.Cin; k.v[1] = g.pad; k.v[2] = g.KW; k.v[3] = g.KH; k.v[4] = g.stride; k.v[5] = p.kp; k.v[7] = 5;
-        const int kp = p.kp;
-        int rc = cached_map(&p.bmap, k, [&](CUtensorMap* m) {
-            cuuint64_t dims[4] = {(cuuint64_t)g.Cin, (cuuint64_t)g.W, (cuuint64_t)g.H, (cuuint64_t)nimg};
-            cuuint64_t strides[3] = {(cuuint64_t)g.Cin * 4, (cuuint64_t)g.W * g.Cin * 4, (cuuint64_t)g.H * g.W * g.Cin * 4};
-            int lower[2] = {-g.pad, -g.pad};
-            int upper[2] = {g.pad - (g.KW - 1), g.pad - (g.KH - 1)};
-            cuuint32_t estr[4] = {1, (cuuint32_t)g.stride, (cuuint32_t)g.stride, 1};
-            CUresult r = g_encode_im2col(m, CU_TENSOR_MAP_DATA_TYPE_TFLOAT32, 4, (void*)x, dims, strides, lower, upper, 32, kp, estr,
-                                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-            if (r != CUDA_SUCCESS) {
-                set_error("cuTensorMapEncodeIm2col(x for wgrad) failed: %d", (int)r);
-                return (int)CG_ERR_CUDA;
-            }
-            if (g_driver_version <= 13010 && nimg * g.H * g.W * g.Cin * 4 < 131072) reinterpret_cast<uint64_t*>(m)[1] &= ~(1ull << 21);
-            return (int)CG_OK;
-        });
-        if (rc) return rc;
-    }
+    p.x = x; p.dy = dy; p.out = splits == 1 ? dw : (float*)ws;
     p.G = g.G; p.xg_images = g.x_groups == 1 ? 0 : g.B;
-    p.B = g.B; p.P = g.Ho; p.Q = g.Wo; p.Cin = g.Cin; p.Cout = g.Cout; p.KH = g.KH; p.KW = g.KW;
-    p.stride = g.stride; p.pad = g.pad;
-    p.out = p.splits == 1 ? dw : (float*)ws;
-    p.T = WG_NCOLS / p.bn;
-    if (p.T > g.KH * g.KW) p.T = g.KH * g.KW;
-    if (wg_xm(g)) {
-        p.Tm = wg_xm_tm(g);
-        const bool two = wg_two(g) && p.Tm * g.Cout <= WG_NCOLS / 2;  // two co-resident CTAs: 2 x 128 TMEM columns each
-        p.nacc = two ? 1 : 2;
-        int stage_bytes = p.kp * 128 * (2 + 4 * p.Tm);
-        int stages = ((two ? 100 : 200) * 1024) / stage_bytes;
-        if (stages > 8) stages = 8;
-        p.stages = stages;
-        size_t smem = (size_t)stages * stage_bytes + 1024 + (2 * stages + 4) * 8 + 16;
-        static PerDeviceOnce attr3_set;
-        if (attr3_set.first()) {
-            cudaError_t e = cudaFuncSetAttribute(wgrad_xm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-            if (e != cudaSuccess) {
-                set_error("cudaFuncSetAttribute(wgrad_xm_kernel): %s", cudaGetErrorString(e));
-                return CG_ERR_CUDA;
-            }
-        }
-        int rgs = g.KH * g.KW * (g.Cin / 32);
-        long units = (long)g.G * p.splits * ((rgs + p.Tm * 4 - 1) / (p.Tm * 4));
-        const int slots = sm_count_now() * (two ? 2 : 1);
-        int grid = (int)(units < slots ? units : slots);
-        if (getenv("COUNCIL_DEBUG")) fprintf(stderr, "wgrad_xm: units=%ld splits=%d chunk=%ld stages=%d Tm=%d kp=%d\n", units, p.splits, p.chunk, stages, p.Tm, p.kp);
-        launch_k(wgrad_xm_kernel, grid, TC_THREADS, smem, st, p);
-        if (int rc = check_launch("wgrad_xm_kernel")) return rc;
-        if (p.splits > 1) {
-            long n4 = (long)g.G * g.Cout * g.KH * g.KW * g.Cin / 4;
-            launch_k(reduce_splits_tc_kernel, cdiv(n4, 256), 256, 0, st, (const float*)ws, dw, n4, p.splits);
-            return check_launch("reduce_splits_tc");
-        }
-        return CG_OK;
-    }
-    if (wg_pair(g)) {
-        int stage_bytes = p.kp * 128 * (4 + WG_NCOLS / 64);
-        int stages = (200 * 1024) / stage_bytes;
-        if (stages > 8) stages = 8;
-        p.stages = stages;
-        size_t smem = (size_t)stages * stage_bytes + 1024 + (2 * stages + 4) * 8 + 16;
-        static PerDeviceOnce attr2_set;
-        if (attr2_set.first()) {
-            cudaError_t e = cudaFuncSetAttribute(wgrad_tc2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-            if (e != cudaSuccess) {
-                set_error("cudaFuncSetAttribute(wgrad_tc2_kernel): %s", cudaGetErrorString(e));
-                return CG_ERR_CUDA;
-            }
-        }
-        long units = (long)g.G * (g.Cout / 256) * p.splits * (g.Cin / p.bn) * ((g.KH * g.KW + p.T - 1) / p.T);
-        int pairs = sm_count_now() / 2;
-        int nclusters = (int)(units < pairs ? units : pairs);
-        if (getenv("COUNCIL_DEBUG")) fprintf(stderr, "wgrad_tc2: units=%ld splits=%d chunk=%ld stages=%d T=%d bn=%d kp=%d\n", units, p.splits, p.chunk, stages, p.T, p.bn, p.kp);
-        launch_k(wgrad_tc2_kernel, 2 * nclusters, TC_THREADS, smem, st, p);
-        if (int rc = check_launch("wgrad_tc2_kernel")) return rc;
-        if (p.splits > 1) {
-            long n4 = (long)g.G * g.Cout * g.KH * g.KW * g.Cin / 4;
-            launch_k(reduce_splits_tc_kernel, cdiv(n4, 256), 256, 0, st, (const float*)ws, dw, n4, p.splits);
-            return check_launch("reduce_splits_tc");
-        }
-        return CG_OK;
-    }
-    // two co-resident CTAs per SM (g_wgrad_2cta): 32-pixel stages, two per CTA, one TMEM accumulator stage each -- the MMAs of two
-    // independent units interleave on the tensor pipe
-    const bool two = wg_two(g);
-    p.nacc = two ? 1 : 2;
-    int stage_bytes = p.kp * 128 * (4 + WG_NCOLS / 32);
-    int stages = ((two ? 100 : 200) * 1024) / stage_bytes;
-    p.stages = stages;
-    size_t smem = (size_t)stages * stage_bytes + 1024 + (2 * stages + 4) * 8 + 16;
+    p.B = g.B; p.H = g.H; p.W = g.W; p.Ho = g.Ho; p.Wo = g.Wo; p.Cin = g.Cin; p.Cout = g.Cout;
+    p.KH = g.KH; p.KW = g.KW; p.stride = g.stride; p.pad = g.pad;
+    p.Mpix = (long)g.B * g.Ho * g.Wo;
+    const int bm = wg_bm(g), bn = wg_bn(g);
+    p.ci_tiles = cdiv(g.Cin, bn);
+    void (*kern)(WgParams) = bm == 128 ? (bn == 128 ? wgrad_tc_kernel<128, 128> : wgrad_tc_kernel<128, 64>)
+                                       : (bn == 128 ? wgrad_tc_kernel<64, 128> : wgrad_tc_kernel<64, 64>);
+    const size_t smem = 2 * (size_t)(bm + bn) * 128 + 1024;
     static PerDeviceOnce attr_set;
     if (attr_set.first()) {
-        cudaError_t e = cudaFuncSetAttribute(wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        if (e != cudaSuccess) {
-            set_error("cudaFuncSetAttribute(wgrad_tc_kernel): %s", cudaGetErrorString(e));
-            return CG_ERR_CUDA;
+        void (*all[4])(WgParams) = {wgrad_tc_kernel<128, 128>, wgrad_tc_kernel<128, 64>, wgrad_tc_kernel<64, 128>, wgrad_tc_kernel<64, 64>};
+        for (auto k : all) {
+            cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 256 * 128 + 1024);
+            if (e != cudaSuccess) {
+                attr_set.reset();
+                set_error("cudaFuncSetAttribute(wgrad_tc_kernel): %s", cudaGetErrorString(e));
+                return CG_ERR_CUDA;
+            }
         }
     }
-    long units = (long)g.G * ((g.Cout + 127) / 128) * p.splits * (g.Cin / p.bn) * ((g.KH * g.KW + p.T - 1) / p.T);
-    const int slots = sm_count_now() * (two ? 2 : 1);
-    int grid = (int)(units < slots ? units : slots);
-    launch_k(wgrad_tc_kernel, grid, TC_THREADS, smem, st, p);
+    launch_k(kern, dim3(p.ci_tiles * g.KH * g.KW, cdiv(g.Cout, bm), g.G * splits), 2 * bm, smem, st, p);
     if (int rc = check_launch("wgrad_tc_kernel")) return rc;
-    if (p.splits > 1) {
+    if (splits > 1) {
         long n4 = (long)g.G * g.Cout * g.KH * g.KW * g.Cin / 4;
-        launch_k(reduce_splits_tc_kernel, cdiv(n4, 256), 256, 0, st, (const float*)ws, dw, n4, p.splits);
+        launch_k(reduce_splits_tc_kernel, cdiv(n4, 256), 256, 0, st, (const float*)ws, dw, n4, splits);
         return check_launch("reduce_splits_tc");
     }
     return CG_OK;

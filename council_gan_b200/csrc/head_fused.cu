@@ -8,10 +8,10 @@
 // pass, three such passes per iteration (dis_update, dis_council_update x2; the pass of gen_update keeps its activations for the
 // backward and stays unfused).  Fused, the 64-channel map is read once and 8 floats per pixel are written.
 //
-// One CTA = 128 threads = 128 pixels per tile, three co-resident CTAs per SM hide each other's latencies.  All threads
-// gather / transform the tile into the K-major 128-byte-swizzled shared-memory operand (TF32-rounded), one thread issues the
-// tcgen05 MMAs (accumulators in TMEM), all threads read the accumulator back (tcgen05.ld), apply bias + ReLU and write the
-// next layer's operand into the same shared-memory tile.  The three weight matrices of the CTA's council member stay resident.
+// One CTA = 128 threads = one warpgroup = 128 pixels per tile, three co-resident CTAs per SM hide each other's latencies.  All
+// threads gather / transform the tile into the K-major 128-byte-swizzled shared-memory operand (TF32-rounded), the warpgroup
+// issues the wgmma MMAs (two 64-row halves, accumulators in registers), applies bias + ReLU and writes the next layer's operand
+// into the same shared-memory tile.  The three weight matrices of the CTA's council member stay resident.
 #include "common.cuh"
 #include "tc_ptx.cuh"
 
@@ -53,8 +53,6 @@ __global__ void __launch_bounds__(HD_THREADS, 3) head_fused_kernel(const HeadP p
     float* s_b1 = reinterpret_cast<float*>(sW3 + HD_W3);  // 64
     float* s_b2 = s_b1 + 64;                               // 64
     float* s_b3 = s_b2 + 64;                               // 16
-    uint64_t* bar = reinterpret_cast<uint64_t*>(s_b3 + 16);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar + 1);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int g = blockIdx.x % p.G, cidx = blockIdx.x / p.G;
@@ -68,70 +66,54 @@ __global__ void __launch_bounds__(HD_THREADS, 3) head_fused_kernel(const HeadP p
         s_b2[threadIdx.x] = __ldg(p.b2 + g * 64 + threadIdx.x);
     }
     if (threadIdx.x < 16) s_b3[threadIdx.x] = threadIdx.x < 12 ? __ldg(p.b3 + g * 12 + threadIdx.x) : 0.f;
-    if (warp == 0) {
-        if (lane == 0) {
-            mbar_init(bar, 1);
-            fence_barrier_init();
-        }
-        __syncwarp();
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(128));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    fence_proxy_async();
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t d_main = tmem_base, d_head = tmem_base + 64;
-    const uint32_t idesc64 = make_idesc_tf32(64), idesc16 = make_idesc_tf32(16);
     const uint64_t desc_hi = make_kmajor_sw128_desc(0);
     const uint32_t a_addr = smem_u32(sA);
-    uint32_t phase = 0;
 
     // loader mapping (coalesced: 8 threads read one 128-byte line): 16-byte unit u of rows r0, r0 + 16, ...
     const int u = threadIdx.x & 7, r0 = threadIdx.x >> 3;
-    // accumulator mapping: thread = pixel row of the tile (TMEM lane), warp w reads lanes 32 w .. 32 w + 31
-    const int row = threadIdx.x;
-    const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
+    // accumulator mapping (wgmma): rows 64 h + 16 warp + lane / 4 (+ 8) of half h, columns 8 j + 2 (lane % 4) (+ 1)
+    const int arow = warp * 16 + (lane >> 2), acol = 2 * (lane & 3);
+    const int row = threadIdx.x;  // pixel row of the mask head
+    float acc[2][32];
+    float hacc[2][8];
 
-    auto issue = [&](uint32_t w_addr, int w_chunk_bytes, uint32_t d_tmem, uint32_t idesc) {
-        // D[128 x N] = A[128 x 64] * W^T: K = 64 = 2 chunks x 4 steps of 8
+    // D[128 x N] = A[128 x 64] * W^T: K = 64 = 2 chunks x 4 steps of 8, for both 64-row halves of the tile
+    auto issue64 = [&](uint32_t w_addr) {
         fence_proxy_async();
-        tc_fence_before();
         __syncthreads();
-        if (threadIdx.x == 0) {
-            tc_fence_after();
+        wgmma_fence();
+#pragma unroll
+        for (int h = 0; h < 2; h++)
 #pragma unroll
             for (int q = 0; q < 8; q++) {
                 const int j = q >> 2, kk = q & 3;
-                const uint64_t adesc = (desc_hi | (uint64_t)(((a_addr + j * 16384) & 0x3FFFF) >> 4)) + (uint64_t)(kk * 2);
-                const uint64_t bdesc = (desc_hi | (uint64_t)(((w_addr + j * w_chunk_bytes) & 0x3FFFF) >> 4)) + (uint64_t)(kk * 2);
-                umma_tf32(d_tmem, adesc, bdesc, idesc, q != 0 ? 1u : 0u);
+                const uint64_t adesc = (desc_hi | (uint64_t)(((a_addr + j * 16384 + h * 8192) & 0x3FFFF) >> 4)) + (uint64_t)(kk * 2);
+                const uint64_t bdesc = (desc_hi | (uint64_t)(((w_addr + j * 8192) & 0x3FFFF) >> 4)) + (uint64_t)(kk * 2);
+                wgmma_tf32<64>(acc[h], adesc, bdesc, q != 0 ? 1 : 0);
             }
-            umma_commit(bar);
-        }
-        mbar_wait(bar, phase);
-        phase ^= 1;
-        tc_fence_after();
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_reg_fence(acc[0], 32);
+        wgmma_reg_fence(acc[1], 32);
+        __syncthreads();  // every MMA reading the tile has retired before it is overwritten
     };
-    // accumulator (64 columns) + bias, ReLU, TF32 -> the shared-memory operand of the next layer (row = this thread)
+    // accumulator + bias, ReLU, TF32 -> the shared-memory operand of the next layer
     auto relayer = [&](const float* bias) {
-        uint8_t* dst = sA + (row >> 3) * 1024 + (row & 7) * 128;
-        const int sw = row & 7;
 #pragma unroll
-        for (int c0 = 0; c0 < 64; c0 += 32) {
-            float v[32];
-            tmem_ld32(d_main + lane_base + (uint32_t)c0, v);
+        for (int h = 0; h < 2; h++)
 #pragma unroll
-            for (int q = 0; q < 8; q++) {
-                float4 o;
-                o.x = fmaxf(v[4 * q] + bias[c0 + 4 * q], 0.f);
-                o.y = fmaxf(v[4 * q + 1] + bias[c0 + 4 * q + 1], 0.f);
-                o.z = fmaxf(v[4 * q + 2] + bias[c0 + 4 * q + 2], 0.f);
-                o.w = fmaxf(v[4 * q + 3] + bias[c0 + 4 * q + 3], 0.f);
-                *reinterpret_cast<float4*>(dst + (c0 >> 5) * 16384 + ((q ^ sw) << 4)) = to_tf32(o);
+            for (int e = 0; e < 2; e++) {
+                const int r = h * 64 + arow + 8 * e;
+                uint8_t* dst = sA + (r >> 3) * 1024 + (r & 7) * 128;
+#pragma unroll
+                for (int j = 0; j < 8; j++) {
+                    const int c = 8 * j + acol;
+                    float2 o;
+                    o.x = to_tf32(fmaxf(acc[h][4 * j + 2 * e] + bias[c], 0.f));
+                    o.y = to_tf32(fmaxf(acc[h][4 * j + 2 * e + 1] + bias[c + 1], 0.f));
+                    *reinterpret_cast<float2*>(dst + (c >> 5) * 16384 + ((((c & 31) >> 2) ^ (r & 7)) << 4) + (c & 3) * 4) = o;
+                }
             }
-        }
     };
 
     for (int tile = cidx; tile < tiles; tile += p.cpg) {
@@ -175,16 +157,45 @@ __global__ void __launch_bounds__(HD_THREADS, 3) head_fused_kernel(const HeadP p
                 *reinterpret_cast<float4*>(dst + j * 16384) = to_tf32(o);
             }
         }
-        issue(smem_u32(sW1), 8192, d_main, idesc64);   // dec.model.7: 1x1 64->64
+        issue64(smem_u32(sW1));   // dec.model.7: 1x1 64->64
         relayer(s_b1);
-        issue(smem_u32(sW2), 8192, d_main, idesc64);   // dec.model.8: 1x1 64->64
+        issue64(smem_u32(sW2));   // dec.model.8: 1x1 64->64
         relayer(s_b2);
-        issue(smem_u32(sW3), 2048, d_head, idesc16);   // dec.model.9: 1x1 64->12 (N padded to 16), tanh below
-        // ---- mask head (networks.py:398-407): h = tanh(.), [o0 rgb | o1 rgb | o2 rgb | m0 m1 m2]
-        float h[16];
-        tmem_ld16(d_head + lane_base, h);
+        // dec.model.9: 1x1 64->12 (N padded to 16), tanh below
+        fence_proxy_async();
+        __syncthreads();
+        wgmma_fence();
 #pragma unroll
-        for (int j = 0; j < 12; j++) h[j] = tanhf(h[j] + s_b3[j]);
+        for (int hh = 0; hh < 2; hh++)
+#pragma unroll
+            for (int q = 0; q < 8; q++) {
+                const int j = q >> 2, kk = q & 3;
+                const uint64_t adesc = (desc_hi | (uint64_t)(((a_addr + j * 16384 + hh * 8192) & 0x3FFFF) >> 4)) + (uint64_t)(kk * 2);
+                const uint64_t bdesc = (desc_hi | (uint64_t)(((smem_u32(sW3) + j * 2048) & 0x3FFFF) >> 4)) + (uint64_t)(kk * 2);
+                wgmma_tf32<16>(hacc[hh], adesc, bdesc, q != 0 ? 1 : 0);
+            }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_reg_fence(hacc[0], 8);
+        wgmma_reg_fence(hacc[1], 8);
+        __syncthreads();
+        // the 16 head columns of a pixel are spread over four lanes: regroup them per row through the (now free) tile
+        float* s_h = reinterpret_cast<float*>(sA);  // [128][17]
+#pragma unroll
+        for (int hh = 0; hh < 2; hh++)
+#pragma unroll
+            for (int e = 0; e < 2; e++)
+#pragma unroll
+                for (int j = 0; j < 2; j++) {
+                    const int r = hh * 64 + arow + 8 * e;
+                    s_h[r * 17 + 8 * j + acol] = hacc[hh][4 * j + 2 * e];
+                    s_h[r * 17 + 8 * j + acol + 1] = hacc[hh][4 * j + 2 * e + 1];
+                }
+        __syncthreads();
+        // ---- mask head (networks.py:398-407): h = tanh(.), [o0 rgb | o1 rgb | o2 rgb | m0 m1 m2]
+        float h[12];
+#pragma unroll
+        for (int j = 0; j < 12; j++) h[j] = tanhf(s_h[row * 17 + j] + s_b3[j]);
         const long pix = m0 + row;                       // pixel within the member
         const float4 xi = hd_ldg4(p.x_img + (pix % ((long)p.B * p.HW)) * 4);
         float im[3] = {xi.x, xi.y, xi.z};
@@ -198,13 +209,7 @@ __global__ void __launch_bounds__(HD_THREADS, 3) head_fused_kernel(const HeadP p
         const long o = ((long)g * p.B * p.HW + pix) * 4;
         *reinterpret_cast<float4*>(p.x_fake + o) = make_float4(im[0], im[1], im[2], 0.f);
         *reinterpret_cast<float4*>(p.mask + o) = make_float4(mk[0], mk[1], mk[2], 0.f);
-        tc_fence_before();  // the next tile's first MMA overwrites d_main / the shared tile only after the barrier inside issue()
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(128));
+        __syncthreads();  // the next tile's gather overwrites the regrouped head outputs
     }
 }
 
@@ -224,7 +229,7 @@ extern "C" int cg_head_fused(const float* y, const float* mean, const float* rst
     p.cpg = 3 * sms / G;
     const long tiles = (long)B * HW / 128;
     if (p.cpg > tiles) p.cpg = (int)tiles;
-    const size_t smem = HD_A + 2 * HD_W + HD_W3 + (64 + 64 + 16) * 4 + 8 + 16 + 1024;
+    const size_t smem = HD_A + 2 * HD_W + HD_W3 + (64 + 64 + 16) * 4 + 1024;
     static PerDeviceOnce attr_once;
     if (attr_once.first()) {
         cudaError_t e = cudaFuncSetAttribute(head_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

@@ -399,7 +399,8 @@ extern "C" int cg_gen_loss_bwd(const cg_gen_loss_desc* d, const cg_gen_loss_hp* 
     int map_blocks = d->n_cl * d->G;
     long total_px = d_mask ? (long)d->G * d->B * d->H * d->W : 0;
     int px_blocks = d_mask ? cdiv(total_px, 256) : 0;
-    if (px_blocks > 148 * 8) px_blocks = 148 * 8;  // grid-stride: each block pays the finalise prologue once
+    const int px_cap = 8 * (tc_sm_count() > 0 ? tc_sm_count() : 1);  // grid-stride: each block pays the finalise prologue once
+    if (px_blocks > px_cap) px_blocks = px_cap;
     int blocks = map_blocks + px_blocks;
     if (blocks == 0) blocks = 1;  // the finalise / publish step always runs
     launch_k(gen_loss_bwd_kernel, blocks, 256, 0, ST, *d, *hp, scal, hist_gan, hist_council, total, ws_total64(ws), accumulate, pub, d_mask,

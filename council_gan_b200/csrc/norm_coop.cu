@@ -25,8 +25,7 @@ constexpr int NC_U1 = 8;  // rows in flight per thread in the forward reduction 
 __device__ __forceinline__ float4 ld_cg4(const float* p) { return __ldcg(reinterpret_cast<const float4*>(p)); }
 
 // L2 eviction priorities: the tensors that are re-read by the second pass are loaded "evict_last" in the first pass, everything
-// that streams through once (residual, second-pass reads, outputs) "evict_first", so the streams do not push the re-read data out
-// (first measurement without hints: 5 % L2 hit rate, the second pass went to HBM again -- profiles/r02_runB_*).
+// that streams through once (residual, second-pass reads, outputs) "evict_first", so the streams do not push the re-read data out.
 __device__ __forceinline__ uint64_t l2_policy_last() {
     uint64_t p;
     asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));

@@ -430,7 +430,8 @@ extern "C" int cg_adam_step(float* p, const float* g, float* m, float* v, long n
     double bc1 = 1.0 - pow((double)beta1, step), bc2 = 1.0 - pow((double)beta2, step);
     float lr_c1 = (float)((double)lr / bc1), rsq_c2 = (float)(1.0 / sqrt(bc2));
     int blocks = cdiv(n, 256);
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    const int cap = 16 * (tc_sm_count() > 0 ? tc_sm_count() : 1);
+    if (blocks > cap) blocks = cap;
     launch_k(adam_kernel, blocks, 256, 0, ST, p, g, m, v, n, lr_c1, beta1, beta2, eps, weight_decay, rsq_c2, grad_scale);
     return check_launch("adam");
 }

@@ -1,6 +1,6 @@
 """Council-stacked networks: AdaIN generator, multi-scale PatchGAN discriminator, council discriminator.
 
-B200-first restructuring of the reference's ``networks.py``: instead of N independent ``nn.Module``
+GPU-first restructuring of the reference's ``networks.py``: instead of N independent ``nn.Module``
 copies executed one after the other (trainer_council.py:101-119, loops at :328,558,747,826,858), the N
 council members of one family live in ONE flat fp32 parameter buffer (stacked ``[N, ...]`` per layer) and
 every layer is ONE grouped kernel launch over all members.  Forward *and* backward are written out
@@ -237,13 +237,11 @@ class CouncilGen(_StackedNet):
         assert g['pad_type'] == 'zero' and g['activ'] == 'relu'
         assert input_dim == 3 and g['num_of_mask_dim_to_add'] == 3, 'mask head kernel is specialised for RGB + 3 masks'
         self.ops, self.hp, self.G = ops, hp, G
-        # statistics in the convolution epilogue (cg_conv_fwd_stats) vs a separate pass; see profiles/r01_summary.md
+        # statistics in the convolution epilogue (cg_conv_fwd_stats) vs a separate pass.
         # '1': every normalised layer; 'auto' (default): the wide layers (>= 128 output channels, K >= 1024), whose main loop is an order of
-        # magnitude longer than the epilogue and hides the reduction; '0': never.  Round 1 measured +5.2 ms with '1' (narrow 256x256 layers
-        # are epilogue-bound); the CTA-pair kernel that serves the wide layers gained the statistics epilogue in round 2.
+        # magnitude longer than the epilogue and hides the reduction; '0': never (the narrow full-resolution layers are epilogue-bound).
         self.fuse_stats = os.environ.get('COUNCIL_FUSE_STATS', 'auto')
-        # single-launch normalisation with L2-resident second pass (csrc/norm_coop.cu): correct and tested, but measured equal to the
-        # two- / three-kernel forms inside the step (profiles/r02_runB_*), so it is opt-in: COUNCIL_COOP_NORM=1
+        # single-launch normalisation with L2-resident second pass (csrc/norm_coop.cu): correct and tested, opt-in: COUNCIL_COOP_NORM=1
         coop = os.environ.get('COUNCIL_COOP_NORM', '0')  # 0 | 1 (forward and backward) | bwd (backward only: keeps the statistics epilogue)
         self.coop_norm = coop == '1'
         self.coop_norm_bwd = coop in ('1', 'bwd')

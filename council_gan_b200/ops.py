@@ -1,7 +1,7 @@
 """ctypes binding of libcouncil_b200.so (the C ABI declared in include/council_b200.h).
 
 PyTorch is used here for device memory (``torch.empty``), the current CUDA stream and nothing else:
-every method hands raw device pointers to a hand-written sm_100a kernel.  There is NO fallback:
+every method hands raw device pointers to a hand-written sm_90a kernel.  There is NO fallback:
 if the shared library is missing or no CUDA device is present, constructing :class:`CudaOps` raises.
 
 Tensor conventions (see the header): fp32, channels-last activations stacked over the council
@@ -122,7 +122,7 @@ class CudaOps:
 
     def __init__(self, device='cuda:0', workspace_bytes=256 << 20):
         if not torch.cuda.is_available():
-            raise RuntimeError('council_gan_b200 needs a CUDA device (sm_100a); no CPU path exists')
+            raise RuntimeError('council_gan_b200 needs a CUDA device (sm_90a); no CPU path exists')
         self.lib = load_library()
         self._stream_cached = None
         self.device = torch.device(device)
@@ -132,8 +132,8 @@ class CudaOps:
         if rc < 0:
             raise RuntimeError('cg_device_info: ' + self.lib.cg_last_error().decode())
         self.sm_count, self.cc = sm.value, (maj.value, mnr.value)
-        if self.cc[0] != 10:
-            raise RuntimeError('libcouncil_b200.so is built for sm_100a only; device is sm_%d%d' % self.cc)
+        if self.cc != (9, 0):
+            raise RuntimeError('libcouncil_b200.so is built for sm_90a only; device is sm_%d%d' % self.cc)
         self._ws = torch.empty(workspace_bytes, dtype=torch.uint8, device=self.device)
         # dedicated, zero-initialised scratch of the fused loss kernels (ticket counter + partial sums); grown on demand
         self._loss_ws = self._zero_bytes(1 << 16)
@@ -154,8 +154,8 @@ class CudaOps:
         return c if c is not None else torch.cuda.current_stream(self.device).cuda_stream
 
     def pin_stream(self):
-        """Resolve torch's current stream ONCE for a run of launches (the trainer pins it for the duration of an update: the lookup
-        was 19 % of the host time of a step on the launch-bound 128x128 configuration, profiles/r02_runM_host_profile_glasses.txt)."""
+        """Resolve torch's current stream ONCE for a run of launches (the trainer pins it for the duration of an update: a per-launch
+        lookup is a noticeable share of the host time of a step on the launch-bound small configurations)."""
         self._stream_cached = torch.cuda.current_stream(self.device).cuda_stream
 
     def unpin_stream(self):
@@ -422,7 +422,7 @@ class CudaOps:
         return x_fake, mask
 
     def head_fused_supported(self, y_shape):
-        # a tcgen05 (TF32) kernel: not used when the exact-fp32 SIMT mode is selected (cg_set_tensor_core_mode(0))
+        # a wgmma (TF32) kernel: not used when the exact-fp32 SIMT mode is selected (cg_set_tensor_core_mode(0))
         return (self._tc_mode & 1) == 1 and y_shape[-1] == 64 and (y_shape[2] * y_shape[3]) % 128 == 0
 
     def mask_head_bwd(self, h, x_in, d_xfake, d_mask=None):

@@ -9,7 +9,7 @@ Same constructor, method names, argument meaning, attribute names and error beha
     trainer.gen_update(images_a, images_b, config, iterations)
     trainer.update_learning_rate()
 
-What is different underneath (B200-first, see DESIGN.md):
+What is different underneath (GPU-first, see DESIGN.md):
   * the N council members are stacked: one grouped kernel launch per layer serves all of them
     (the reference loops ``for i in range(self.council_size)`` in Python, :328,558,747,826,858);
   * forward and backward are explicit sequences of our own CUDA kernels; no autograd graph, no
@@ -66,7 +66,7 @@ def _pinned(fn):
         ops.pin_stream()
         if _PDL != 'auto':
             ops.set_pdl(_PDL == '1')
-        else:  # launch-bound small maps only (measured: -4 % at 128x128 x 1, +2 % at 256x256 x 8)
+        else:  # launch-bound small maps only: early-scheduled dependents cost more than the launch gaps they hide once kernels are long
             for x in args:
                 if torch.is_tensor(x):
                     pix = x.numel() // (IMG_C if x.dim() == 5 else max(int(x.shape[1]), 1)) if x.dim() >= 4 else 0

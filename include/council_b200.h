@@ -1,5 +1,5 @@
 /*
- * council_b200.h -- C ABI of libcouncil_b200.so: the sm_100a kernels behind the Council-GAN
+ * council_b200.h -- C ABI of libcouncil_b200.so: the sm_90a kernels behind the Council-GAN
  * training step (dis_update / dis_council_update / gen_update).
  *
  * The reference (Onr/Council-GAN) has no FFI: every device op on this path is a PyTorch library
@@ -34,7 +34,7 @@ typedef enum {
     CG_ERR_ARG = -1,        /* unsupported shape / argument */
     CG_ERR_WORKSPACE = -2,  /* workspace too small */
     CG_ERR_CUDA = -3,       /* CUDA runtime / driver error */
-    CG_ERR_NO_DEVICE = -4   /* no sm_100 device */
+    CG_ERR_NO_DEVICE = -4   /* no CUDA device */
 } cg_status;
 
 /* activation codes (Conv2dBlock activations, networks.py:494-507) */
@@ -54,18 +54,12 @@ typedef struct {
 const char* cg_last_error(void);
 /* Library / device introspection: returns the SM count of the current device (>0) or a cg_status. */
 int cg_device_info(int* sm_count, int* cc_major, int* cc_minor);
-/* 0 = SIMT fp32 kernels only; 1 (default) = tcgen05 TF32 tensor-core kernels wherever a layer qualifies;
+/* 0 = SIMT fp32 kernels only; 1 (default) = TF32 tensor-core kernels (wgmma / mma.sync) wherever a layer qualifies;
  * other values are a bit mask for bring-up: 2 = data gradient only, 4 = weight gradient only, ...
- * (internally 1 forward | 2 dgrad | 4 wgrad).  Measurement switches on top of the mask: 8 = no CTA-pair (cta_group::2)
- * kernels, 16 = none for 128-wide tiles, 32 = CTA pairs for 64-wide tiles too, 64 = CTA pairs in the weight
- * gradient too (both measured slower), 1<<16 = one weight-gradient CTA per SM, 1<<18 = one x-on-M weight-gradient CTA per SM and 1<<17 =
- * one forward CTA per SM for tiles <= 64 channels wide (default: two co-resident CTAs interleave their MMAs), 1<<19 = image-side layers (<= 8 input lanes)
- * on the older TMA-im2col / explicit-patch paths instead of the shared-memory patch builders (csrc/conv_img.cu), 1<<20 = accumulator-layout epilogue
- * stores instead of the coalescing shared-memory patch (default: patch for tiles <= 64 channels wide; 1<<21 = for the wide tiles too),
- * 1<<22 = programmatic dependent launch between this library's kernels (every kernel carries the griddepcontrol pair; measured -4 % on the
- * launch-bound 128x128 configuration and +2 % at 256x256 batch 8, so the trainer turns it on for small maps only),
- * 1<<24 = programmatic dependent launch for the helper kernels only (those without dynamic shared memory),
- * 1<<23 = keep the widest N tile on small maps (default: narrower tiles when a launch has fewer tiles than SMs), bits 8..15 = cap on the CTA pairs launched.
+ * (internally 1 forward | 2 dgrad | 4 wgrad).  Switches on top of the mask: 1<<22 = programmatic dependent launch between this
+ * library's kernels (every kernel carries the griddepcontrol pair; the trainer turns it on for small maps only), 1<<24 = programmatic
+ * dependent launch for the helper kernels only (those without dynamic shared memory), 1<<23 = keep the widest N tile on small maps
+ * (default: narrower tiles when a launch has fewer tiles than SMs).  Other bits are accepted and ignored.
  * The switches are per calling thread (like cg_last_error), not process-global.  Returns the previous mask. */
 int cg_set_tensor_core_mode(int mode);
 /* number of kernels launched by this library since load (bench.py reports it as gpu_launches) */

@@ -1,4 +1,4 @@
-"""Bring-up harness for the tcgen05 convolution: each case runs in its own subprocess with a timeout so a
+"""Bring-up harness for the tensor-core convolution: each case runs in its own subprocess with a timeout so a
 hang cannot take the whole GPU visit down; prints error statistics instead of asserting."""
 import json
 import subprocess

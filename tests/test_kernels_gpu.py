@@ -58,7 +58,7 @@ CONV_CASES = [
     ('dis_out_1x1_b32', 4, 4, 32, 32, 32, 512, 1, 1, 1, 0, False),
     ('dis_out_1x1_c256_odd', 3, 3, 5, 7, 9, 256, 1, 1, 1, 0, False),
     ('odd_sizes', 1, 1, 1, 10, 14, 8, 20, 3, 1, 1, False),
-    # shapes that qualify for the tcgen05 path (>= 128 output pixels per member)
+    # shapes that qualify for the tensor-core path (>= 128 output pixels per member)
     ('tc_res_3x3_256', 2, 2, 2, 16, 16, 256, 256, 3, 1, 1, False),
     ('tc_down_4x4s2_64_128', 2, 2, 2, 32, 32, 64, 128, 4, 2, 1, False),
     ('tc_down_4x4s2_256_512', 2, 2, 3, 16, 16, 256, 512, 4, 2, 1, False),
@@ -66,15 +66,14 @@ CONV_CASES = [
     ('tc_dc_1x1_512_512', 3, 3, 4, 8, 8, 512, 512, 1, 1, 0, False),
     ('tc_shared_input', 3, 1, 2, 16, 16, 64, 64, 3, 1, 1, False),
     ('tc_partial_tiles', 2, 2, 3, 12, 20, 64, 128, 3, 1, 1, False),
-    # CTA-pair kernel (Cout % 256 == 0, >= 512 pixels): 640 px = 2.5 pair tiles (second CTA of the last pair idle),
-    # 720 px (partial second CTA), dgrad classes of a stride-2 layer
+    # 256-wide tiles with partial pixel tiles (640 / 720 px), dgrad classes of a stride-2 layer
     ('tc_pair_half_tile', 2, 2, 5, 8, 16, 64, 256, 3, 1, 1, False),
     ('tc_pair_partial', 2, 2, 3, 12, 20, 32, 512, 3, 1, 1, False),
     ('tc_pair_dgrad_s2', 2, 2, 2, 32, 32, 256, 64, 4, 2, 1, False),
-    # CTA-pair weight gradient: 256 output channels per unit; 64- and 192-channel inputs (one / three boxes per CTA and tap)
+    # weight gradient with 256 output channels; 64- and 192-channel inputs (one full / one partial 64-channel tile per tap)
     ('tc_pair_wgrad_c64_o256', 2, 2, 2, 16, 16, 64, 256, 3, 1, 1, False),
     ('tc_pair_wgrad_c192_o256', 1, 1, 2, 16, 16, 192, 256, 3, 1, 1, False),
-    # x-on-M weight gradient (<= 64 output channels): partial last row tile (3x3x64: 18 row groups), 1x1 with 3 row groups
+    # weight gradient with <= 64 output channels: 128 / 96 / 32 input channels (full and partial 64-channel tiles)
     ('tc_xm_wgrad_c128_o64', 2, 2, 2, 16, 16, 128, 64, 3, 1, 1, False),
     ('tc_xm_wgrad_1x1_c96_o64', 2, 1, 2, 16, 16, 96, 64, 1, 1, 0, False),
     ('tc_xm_wgrad_4x4s2_c32_o32', 2, 2, 2, 32, 32, 32, 32, 4, 2, 1, False),
@@ -82,7 +81,7 @@ CONV_CASES = [
     ('patch_disc0_3x3_pair', 2, 2, 2, 16, 16, 8, 64, 3, 1, 1, False),
     ('patch_dis0_4x4s2_img', 2, 2, 4, 16, 16, 4, 64, 4, 2, 1, False),
     ('patch_enc0_7x7_shared', 3, 1, 2, 16, 16, 4, 64, 7, 1, 3, False),
-    # shared-memory patch builder: several tiles per CTA, image borders inside tiles, weight-gradient CTAs with no work
+    # image-side layers on larger maps: several tiles per CTA, image borders inside tiles
     ('img_disc0_3x3_pair_multi', 3, 3, 5, 32, 32, 8, 64, 3, 1, 1, False),
     ('img_dis0_4x4s2_rect', 2, 2, 3, 32, 64, 4, 64, 4, 2, 1, False),
 ]
@@ -91,23 +90,12 @@ CONV_CASES = [
 @pytest.mark.parametrize('case', CONV_CASES, ids=[c[0] for c in CONV_CASES])
 @pytest.mark.parametrize('tc', [0, 1, 7 | 32 | 64 | (1 << 16), 7 | (1 << 17), 7 | (1 << 19), 7 | (1 << 20), 7 | (1 << 21), 7 | (1 << 22), 7 | (1 << 23)])
 def test_conv_fwd_dgrad_wgrad(ops, ref, case, tc):
-    """tc = 0: SIMT fp32; 1: the default tensor-core dispatch; 7|32|64|1<<16: the switchable variants that are off by default --
-    CTA pairs (cta_group::2) for 64-wide forward tiles and in the weight gradient, one weight-gradient CTA per SM instead of the default two;
-    7|1<<17: ONE forward / data-gradient CTA per SM for tiles <= 64 channels wide (the default co-schedules two);
-    7|1<<20: accumulator-layout epilogue stores everywhere (the default sends tiles <= 64 channels wide through the coalescing
-    shared-memory patch); 7|1<<21: the patch on the wide tiles too; 7|1<<22: programmatic dependent launch; 7|1<<23: widest N tile even on small maps (the default narrows
-    the tile when a launch has fewer tiles than SMs -- which these test shapes do, so tc=1 exercises the narrowed tiles and this one the wide)."""
+    """tc = 0: SIMT fp32; 1: the default tensor-core dispatch; the other masks add switch bits to the full mask (see
+    cg_set_tensor_core_mode in include/council_b200.h: 1<<22 programmatic dependent launch, 1<<23 widest N tile even on small maps --
+    the default narrows the tile when a launch has fewer tiles than SMs, which these test shapes do, so tc=1 exercises the narrowed
+    tiles and this one the wide; bits the library ignores must leave every result unchanged).  Every mode runs on every
+    geometry: whichever kernels a mode selects for a layer, the results must hold."""
     name, G, Gx, B, H, W, Cin, Cout, K, stride, pad, ups = case
-    if tc == 7 | (1 << 19):
-        # image-side layers: the default is the shared-memory patch builder (csrc/conv_img.cu); bit 19 selects the older
-        # TMA-im2col forward / explicit-patch weight gradient, which stay tested
-        if not (Cin <= 8 and Cout == 64 and K * K * Cin <= 96):
-            pytest.skip('not an image-side layer')
-    elif tc in (7 | (1 << 20), 7 | (1 << 21), 7 | (1 << 22), 7 | (1 << 23)):
-        if not name.startswith('tc_'):
-            pytest.skip('not a tensor-core forward / data-gradient geometry')
-    elif tc > 1 and not (name.startswith('tc_') and (Cout % 128 == 0 or Cout <= 64 or Cin <= 64)):
-        pytest.skip('no optional variant for this geometry')
     ops.set_tensor_core_mode(tc)
     tol = 2e-5 if tc == 0 else 4e-3
     try:
@@ -150,7 +138,7 @@ STATS_CASES = [
     ('stats_up_classes', 2, 2, 2, 16, 16, 128, 64, 3, 1, 1, True),
     ('stats_first_7x7_patch', 2, 1, 2, 16, 16, 4, 64, 7, 1, 3, False),
     ('stats_small_map_simt', 2, 2, 1, 8, 8, 256, 256, 3, 1, 1, False),
-    # CTA-pair kernel with the statistics epilogue (round 2): 256- and 128-wide tiles, the production residual-block shape
+    # statistics epilogue on 256- and 128-wide tiles, the production residual-block shape
     ('stats_pair_128_wide', 2, 2, 2, 32, 32, 128, 128, 3, 1, 1, False),
     ('stats_pair_down_128_256', 2, 2, 2, 32, 32, 128, 256, 4, 2, 1, False),
     ('stats_prod_res_3x3_256', 4, 4, 8, 64, 64, 256, 256, 3, 1, 1, False),
@@ -274,7 +262,7 @@ def test_mask_head(ops, ref):
 @pytest.mark.parametrize('shape', [(2, 2, 16, 16), (4, 8, 256, 256), (3, 1, 8, 48)])
 @pytest.mark.parametrize('adain_on', [True, False])
 def test_head_fused(ops, ref, shape, adain_on):
-    """cg_head_fused (AdaIN + ReLU -> 1x1 -> 1x1 -> 1x1 tanh -> mask compositing in one tcgen05 kernel) against the float64
+    """cg_head_fused (AdaIN + ReLU -> 1x1 -> 1x1 -> 1x1 tanh -> mask compositing in one wgmma kernel) against the float64
     composition of the separate ops, and against the separate CUDA ops it replaces."""
     G, B, H, W = shape
     y = rnd(G, B, H, W, 64, seed=1, scale=1.5) + 0.2

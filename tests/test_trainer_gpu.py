@@ -58,7 +58,7 @@ def check_iteration(case, tc):
     if tc == 0:
         wg, wp = compare_with_oracle(tr, orc, hp, rtol_loss=1e-3, grad_rel_l2=3e-2, flip_frac=0.03, min_cos=0.999)
     else:
-        # TF32 operands: scripts/grad_noise.py (profiles/r01_grad_noise.log) shows that perturbing the WEIGHTS by
+        # TF32 operands: scripts/grad_noise.py shows that perturbing the WEIGHTS by
         # 2^-11 relative noise with exact fp32 kernels already moves the deep generator gradients by 15 % (cos 0.989)
         # -- the same as the tensor-core path does (13.5 %, cos 0.991) -- and with the focus loss live
         # (sign(m-.5)/(|m-.5|+eps)^2 on masks that start at ~0.5) the gradient is discontinuous in the mask.  So the
@@ -212,7 +212,7 @@ def test_baseline_configuration_vs_reference_golden(case):
                     assert abs(a - b) <= 2.1 * lr + 1e-6, (fam, i, key, a, b)
                 assert abs(got['absmean'] - rec['post']['absmean']) <= 1.0 * lr + 1e-4 * abs(rec['post']['absmean']), (fam, i, key)
                 # gradient norm of the head layer: only without focus loss -- sign(m-.5)/(|m-.5|+eps)^2 on masks near 0.5 makes the
-                # gradient discontinuous in the mask (TF32 vs fp32 pixels flip sides; profiles/r01_grad_noise.log)
+                # gradient discontinuous in the mask (TF32 vs fp32 pixels flip sides; scripts/grad_noise.py)
                 if fam == 'gen' and 'grad' in rec and not gold['loss_gen_mask_zero_one'] and key in ('dec.model.9.conv.weight', 'dec.model.9.conv.bias'):
                     g = tr._nets['gen_' + d0]
                     spec = [s for s in g._specs() if key in (s.wname, s.bname)][0]
