@@ -15,6 +15,7 @@ extern std::atomic<uint64_t> g_launches;
 // kernel-selection switches of cg_set_tensor_core_mode: per calling THREAD (like cg_last_error), not process-global
 extern thread_local int g_tc_mode;
 extern thread_local int g_small_bn;
+extern thread_local int g_wgrad_tma;
 
 constexpr int CG_MAX_DEVICES = 64;
 inline int current_device() {

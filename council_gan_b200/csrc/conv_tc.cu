@@ -21,6 +21,7 @@
 // Kernels in this file (host dispatch at the bottom of each section):
 //   conv_tc_kernel<BK, BN>  forward / data gradient
 //   wgrad_tc_kernel<BM, BN> weight gradient (MN-major operands transposed in shared memory, then wgmma)
+//   wgrad_tma_kernel<BM, BN> weight gradient of stride-1 KxK layers (TMA-fed, shifted operand from registers)
 //
 // Reference call sites replaced: nn.Conv2d forward (networks.py:513,516) and cuDNN dgrad via autograd.
 #include "common.cuh"
@@ -866,7 +867,346 @@ static void wg_plan(const cg_conv_geom& g, int& splits, long& chunk) {
     splits = (int)((Mpix + chunk - 1) / chunk);
 }
 
+// ------------------------------------------------------------------------------------------------
+// weight gradient of stride-1 convolutions with KH*KW > 1: TMA-fed wgmma pipeline, shifted operand from registers
+//
+// For tap k = (kh, kw) and stride 1,  dW[k][co][ci] = sum over x pixels p of dy[p - k + pad][co] * x[p][ci]
+//                                                    = sum over dy pixels o of x[o + k - pad][ci] * dy[o][co],
+// out-of-range x pixels counting as zero.  The reduction (K) runs over dy pixels, x is read at tap-shifted pixels.
+// * dy is "copied": a transpose kernel writes it channel-major [img][Cout][Ho][Wo], TF32-rounded, into the workspace once per
+//   call, and a 4-D tiled map (W, H, C, N) with a (32 px, 1, BN channels, 1) box brings 32 pixels of one row straight into the
+//   K-major 128-byte-swizzled layout wgmma reads as its B operand.  Chunk starts are multiples of 32 pixels, so the innermost
+//   TMA coordinate stays aligned; a partial last chunk of a row is zero-filled.
+// * x ("direct") is read from its channels-last layout with a (C, W, H, N) map, box (32 channels, 32 px, 1, 1): the tap shift
+//   moves the W and H coordinates, which are outer dimensions, so starts off the map are legal and zero-filled (the padding).
+//   That tile is MN-major, which wgmma cannot take as a TF32 shared-memory operand; the consumers read their A fragments out of
+//   it with LDS, round them to TF32 and issue the register-A ("RS") form of wgmma.
+// * M = Cin, N = Cout: the epilogue stores D transposed into dw[g][co][kh][kw][ci].
+// * Same arithmetic as wgrad_tc_kernel: the same TF32-rounded operands, the same pixel splits (wg_plan), and within a split the
+//   same 8-pixel k-steps in the same order, so where Wo % 32 == 0 (a 32-pixel chunk of dy is 32 consecutive pixels of one row)
+//   both kernels produce the same bits.  Training amplifies any rounding difference in the weight gradients within a few steps,
+//   so a kernel that merely agreed to rounding would change what a training run computes.
+// * Warp-specialised persistent CTAs as in conv_tc_kernel: one TMA producer thread, BM / 64 consumer warpgroups, a full / empty
+//   mbarrier ring.  Work units (pixel split, group, tap, M tile, N tile) are walked split-major, so that the CTAs running at the
+//   same time read the same pixel range and the KH*KW re-reads of it come from L2.  Splits write partials that
+//   reduce_splits_tc_kernel sums in a fixed order (deterministic).
+// ------------------------------------------------------------------------------------------------
+thread_local int g_wgrad_tma = 1;  // mode bit 25 clears it: stride-1 weight gradients stay on wgrad_tc_kernel
+
+constexpr int WT_MAX_STAGES = 8;
+
+struct WtParams {
+    CUtensorMap amap;               // x, channels-last
+    CUtensorMap bmap;               // channel-major copy of dy
+    float* out;                     // [split][G][Cout][KH][KW][Cin]
+    int G, KW, taps, M, N, Cin, Cout;
+    int a_gimg, b_gimg;             // images per group in the x / dy-copy map (0: input shared by the council)
+    int Hc, cpr;                    // dy grid: rows per image, 32-pixel chunks per row
+    int pad;                        // x pixel = dy pixel + tap - pad
+    long chunks, split_chunks;      // chunks per member, per split
+    int units, stages;
+};
+
+// Accumulator row r (0..15) of warp w of a consumer warpgroup <-> channel of the direct tile.  With the 128-byte swizzle, channel c of
+// pixel k sits in 16-byte chunk (c / 4) ^ (k % 8) of the pixel's 128-byte row.  One A-fragment LDS of a warp reads 8 rows at 4
+// consecutive pixels (k % 8 in 0..3 or 4..7); if the 8 rows were 8 consecutive channels they would span 2 chunks, and
+// XOR-ed with 4 pixel values those give only 4 distinct chunks: 2-way bank conflicts.  Rows r = 0..3 -> channels c..c+3 and
+// r = 4..7 -> c+16..c+19 instead come from chunks q and q + 4 (q even), which the XOR keeps apart: 8 chunks, 32 banks.
+// Rows 8..15 take the channels 4 above those of rows 0..7; warps w and w^1 share one 32-channel box.
+// shared-memory load of one A fragment element, rounded to TF32 (the tensor core would truncate it)
+__device__ __forceinline__ uint32_t lds_tf32(uint32_t addr) {
+    float v;
+    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
+    return tf32_bits(v);
+}
+__device__ __forceinline__ int wt_row_channel(int w, int r) { return 32 * (w >> 1) + 8 * (w & 1) + (r & 3) + 16 * ((r >> 2) & 1) + 4 * (r >> 3); }
+
+template <int BM, int BN>
+__global__ void __launch_bounds__(2 * BM + 128, BM == 64 ? 2 : 1) wgrad_tma_kernel(const __grid_constant__ WtParams p) {
+    constexpr int A_BOX = 32 * 128;                // 32 channels x 32 pixels
+    constexpr int STAGE = (BM + BN) * 128;         // [A box 0 .. BM/32-1][B: BN rows of 32 pixels]
+    constexpr int NCW = BM / 64;                   // consumer warpgroups
+    pdl_trigger();
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    const int wg = __shfl_sync(0xffffffffu, threadIdx.x >> 7, 0), tid = threadIdx.x & 127;
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * STAGE);
+    uint64_t* empty_bar = full_bar + p.stages;
+    const int MT = (p.M + BM - 1) / BM, NT = (p.N + BN - 1) / BN;
+
+    if (threadIdx.x == 0) {
+        prefetch_tmap(&p.amap);
+        prefetch_tmap(&p.bmap);
+        for (int s = 0; s < p.stages; s++) {
+            mbar_init(&full_bar[s], 1);
+            mbar_init(&empty_bar[s], NCW);
+        }
+        fence_barrier_init();
+    }
+    __syncthreads();
+    pdl_wait();
+
+    if (wg == 0) {
+        // ===================== TMA producer =====================
+        if (tid == 0) {
+            int stage = 0;
+            uint32_t phase = 0;
+            for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+                int r = u / NT;
+                const int n0 = (u - r * NT) * BN;
+                const int m0 = (r % MT) * BM;
+                r /= MT;
+                const int tap = r % p.taps;
+                r /= p.taps;
+                const int g = r % p.G, split = r / p.G;
+                const int kh = tap / p.KW, kw = tap - kh * p.KW;
+                const int sh = kh - p.pad, sw = kw - p.pad;
+                int nbox = (p.M - m0) / 32;                // whole 32-channel boxes inside the tensor (M % 32 == 0)
+                if (nbox > BM / 32) nbox = BM / 32;       // rows past M are never stored: their boxes are not loaded
+                const uint32_t tx = (uint32_t)(nbox * A_BOX + BN * 128);
+                long c = split * p.split_chunks, c_end = c + p.split_chunks;
+                if (c_end > p.chunks) c_end = p.chunks;
+                const long per_img = (long)p.Hc * p.cpr;
+                int img = (int)(c / per_img);
+                int rem = (int)(c - img * per_img);
+                int h = rem / p.cpr, wq = rem - h * p.cpr;
+                for (; c < c_end; c++) {
+                    mbar_wait(&empty_bar[stage], phase ^ 1);
+                    uint8_t* sa = smem + (size_t)stage * STAGE;
+                    mbar_expect_tx(&full_bar[stage], tx);
+                    const int w0 = wq * 32;
+                    for (int j = 0; j < nbox; j++)
+                        tma_load_4d(&p.amap, &full_bar[stage], sa + j * A_BOX, m0 + 32 * j, w0 + sw, h + sh, g * p.a_gimg + img);
+                    tma_load_4d(&p.bmap, &full_bar[stage], sa + BM * 128, w0, h, n0, g * p.b_gimg + img);
+                    if (++wq == p.cpr) { wq = 0; if (++h == p.Hc) { h = 0; ++img; } }
+                    if (++stage == p.stages) { stage = 0; phase ^= 1; }
+                }
+            }
+        }
+        return;
+    }
+
+    // ===================== MMA + epilogue (consumer warpgroups) =====================
+    const int cw = wg - 1, warp4 = tid >> 5, lane = tid & 31;
+    const int wl = 2 * cw + (warp4 >> 1);                      // this warp's 32-channel box ...
+    const int wsub = warp4 & 1;                                // ... and which half of it (see wt_row_channel)
+    const int ch0 = wt_row_channel(wsub, lane >> 2);            // channel in the box of accumulator row lane / 4; row + 8: ch0 + 4
+    const int kq = lane & 3;
+    // byte offsets of a[0..3] in the box for k-step 0: (ch0, kq), (ch0 + 4, kq), (ch0, kq + 4), (ch0 + 4, kq + 4); k-step kk adds 1024 kk
+    auto swz = [](int ch, int k) { return k * 128 + ((((ch >> 2) ^ (k & 7))) << 4) + (ch & 3) * 4; };
+    const int off0 = swz(ch0, kq) + wl * A_BOX, off1 = swz(ch0 + 4, kq) + wl * A_BOX;
+    const int off2 = swz(ch0, kq + 4) + wl * A_BOX, off3 = swz(ch0 + 4, kq + 4) + wl * A_BOX;
+    const uint64_t desc0 = make_kmajor_sw128_desc(0);
+    const long Ktot = (long)p.taps * p.Cin;
+    float acc[BN / 2];
+    uint32_t af[2][4];
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+        int r = u / NT;
+        const int n0 = (u - r * NT) * BN;
+        const int m0 = (r % MT) * BM;
+        r /= MT;
+        const int tap = r % p.taps;
+        r /= p.taps;
+        const int g = r % p.G, split = r / p.G;
+        long c0 = split * p.split_chunks, c_end = c0 + p.split_chunks;
+        if (c_end > p.chunks) c_end = p.chunks;
+        int prev = -1;
+        for (long c = c0; c < c_end; c++) {
+            mbar_wait(&full_bar[stage], phase);
+            const uint32_t sa32 = smem_u32(smem + (size_t)stage * STAGE);
+            const uint32_t sb = sa32 + BM * 128;
+            const uint64_t bdesc = desc0 | (uint64_t)((sb & 0x3FFFF) >> 4);
+#pragma unroll
+            for (int kk = 0; kk < 4; kk++) {
+                // double-buffered fragments: af[kk & 1] was last read by the MMA of k-step kk - 2, which the wait below retired
+                uint32_t* a = af[kk & 1];
+                a[0] = lds_tf32(sa32 + off0 + 1024 * kk);
+                a[1] = lds_tf32(sa32 + off1 + 1024 * kk);
+                a[2] = lds_tf32(sa32 + off2 + 1024 * kk);
+                a[3] = lds_tf32(sa32 + off3 + 1024 * kk);
+                wgmma_fence();  // orders the fragment writes above (and the accumulators) before the asynchronous MMA reads them
+                wgmma_tf32_rs<BN>(acc, a, bdesc + (uint64_t)(kk * 2), (c != c0 || kk) ? 1 : 0);
+                wgmma_commit();
+                wgmma_wait<1>();  // the MMA of k-step kk - 1 has retired: its fragment buffer is free
+                // at k-step 0 that was the last MMA of the previous chunk: its stage can be refilled
+                if (kk == 0 && prev >= 0 && tid == 0) mbar_arrive(&empty_bar[prev]);
+            }
+            prev = stage;
+            if (++stage == p.stages) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+        wgmma_reg_fence(acc, BN / 2);
+        if (tid == 0) mbar_arrive(&empty_bar[prev]);
+
+        float* out = p.out + ((long)split * p.G + g) * p.Cout * Ktot + (long)tap * p.Cin;
+        const int cq = 2 * (lane & 3);
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const int m = m0 + 32 * wl + ch0 + 4 * h;
+            if (m >= p.M) continue;
+#pragma unroll
+            for (int j = 0; j < BN / 8; j++) {
+                const int n = n0 + 8 * j + cq;
+                if (n >= p.N) break;
+                const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                out[(long)n * Ktot + m] = v0;  // m = ci, n = co
+                out[(long)(n + 1) * Ktot + m] = v1;
+            }
+        }
+    }
+}
+
+// [img][H][W][C] -> [img][C][H][W], rounded to TF32 as wgrad_tc_kernel rounds its operands: 32 pixels x 32 channels per block
+// through a padded shared tile; float4 reads along C, 128-byte writes along W.  grid (W tiles * C tiles, H, images)
+__global__ void __launch_bounds__(256) nhwc_to_nchw_tf32_kernel(const float* __restrict__ src, float* __restrict__ dst, int H, int W, int C) {
+    pdl_trigger();
+    pdl_wait();
+    __shared__ float tile[32][33];
+    const int ct = C / 32;
+    const int w0 = (blockIdx.x / ct) * 32, c0 = (blockIdx.x % ct) * 32;
+    const int h = blockIdx.y;
+    const long img = blockIdx.z;
+    const int t = threadIdx.x;
+    const int px = t >> 3, c4 = (t & 7) * 4;
+    if (w0 + px < W) {
+        const float4 v = __ldg(reinterpret_cast<const float4*>(src + ((img * H + h) * W + w0 + px) * C + c0 + c4));
+        tile[c4][px] = v.x; tile[c4 + 1][px] = v.y; tile[c4 + 2][px] = v.z; tile[c4 + 3][px] = v.w;
+    }
+    __syncthreads();
+    const int tx = t & 31, ty = t >> 5;
+    if (w0 + tx >= W) return;
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+        const int c = ty + 8 * j;
+        dst[((img * C + c0 + c) * H + h) * W + w0 + tx] = to_tf32(tile[c][tx]);
+    }
+}
+
+bool tc_wgrad_tma_supported(const cg_conv_geom& g) {
+    if (!g_wgrad_tma || g.stride != 1 || g.ups || g.KH * g.KW <= 1) return false;
+    if (g.Cin % 32 != 0 || g.Cout % 32 != 0) return false;
+    init_driver();
+    if (!g_encode_tiled) return false;
+    if (g.W < 32 || g.Wo < 32 || g.Wo % 4 != 0) return false;  // Wo % 4: TMA strides of the copy are multiples of 16 bytes
+    return (long)g.B * g.Ho * g.Wo >= 256;
+}
+
+struct WtPlan {
+    int bm, bn, cpr, splits, slots;
+    long chunks, split_chunks, copy_bytes, part_bytes;
+};
+
+static WtPlan wt_plan(const cg_conv_geom& g) {
+    WtPlan q;
+    q.bm = g.Cin > 64 ? 128 : 64;
+    q.bn = q.bm == 64 ? 64 : g.Cout >= 256 ? 256 : g.Cout > 64 ? 128 : 64;
+    q.cpr = cdiv(g.Wo, 32);
+    q.chunks = (long)g.B * g.Ho * q.cpr;
+    q.copy_bytes = (((long)g.G * g.B * g.Ho * g.Wo * g.Cout * 4) + 1023) & ~1023L;
+    q.slots = (q.bm == 64 ? 2 : 1) * sm_count_now();  // two CTAs per SM for the single-warpgroup 64 x 64 tiles
+    // the pixel splits of wgrad_tc_kernel (see the section comment); `chunk` is a multiple of 32 pixels
+    int splits;
+    long chunk;
+    wg_plan(g, splits, chunk);
+    q.split_chunks = g.Wo % 32 == 0 ? chunk / 32 : (q.chunks + splits - 1) / splits;
+    q.splits = (int)((q.chunks + q.split_chunks - 1) / q.split_chunks);
+    q.part_bytes = q.splits > 1 ? (long)q.splits * g.G * g.Cout * g.KH * g.KW * g.Cin * 4 : 0;
+    return q;
+}
+
+template <int BM, int BN>
+static int launch_wt(WtParams& p, int slots, cudaStream_t st) {
+    constexpr int STAGE = (BM + BN) * 128;
+    // 64 x 64 tiles: two CTAs per SM (228 KB of shared memory per SM, 1 KB of it reserved per CTA)
+    int stages = ((BM == 64 ? 110 : 225) * 1024 - 1024 - 2 * WT_MAX_STAGES * 8) / STAGE;
+    if (stages > WT_MAX_STAGES) stages = WT_MAX_STAGES;
+    p.stages = stages;
+    const size_t smem = (size_t)stages * STAGE + 1024 + 2 * stages * 8;
+    static PerDeviceOnce attr_set;
+    if (attr_set.first()) {
+        cudaError_t e = cudaFuncSetAttribute(wgrad_tma_kernel<BM, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) {
+            attr_set.reset();
+            set_error("cudaFuncSetAttribute(wgrad_tma_kernel): %s", cudaGetErrorString(e));
+            return CG_ERR_CUDA;
+        }
+    }
+    const int grid = p.units < slots ? p.units : slots;
+    launch_k(wgrad_tma_kernel<BM, BN>, grid, 2 * BM + 128, smem, st, p);
+    return check_launch("wgrad_tma_kernel");
+}
+
+static int tc_conv_wgrad_tma(const cg_conv_geom& g, const float* x, const float* dy, float* dw, void* ws, cudaStream_t st) {
+    const WtPlan q = wt_plan(g);
+    float* copy = (float*)ws;
+    float* part = (float*)((uint8_t*)ws + q.copy_bytes);
+    const long nimg_x = g.x_groups == 1 ? g.B : (long)g.G * g.B, nimg_dy = (long)g.G * g.B;
+    launch_k(nhwc_to_nchw_tf32_kernel, dim3(q.cpr * (g.Cout / 32), g.Ho, (unsigned)nimg_dy), 256, 0, st, dy, copy, g.Ho, g.Wo, g.Cout);
+    if (int rc = check_launch("nhwc_to_nchw_tf32")) return rc;
+
+    // Both maps move raw fp32 (the copy is already rounded, x is rounded in registers), whatever a TF32 map would do to the low bits.
+    WtParams p{};
+    // x: channels-last (C, W, H, N), box (32 channels, 32 px, 1, 1)
+    {
+        MapKey k{};
+        k.ptr = x; k.a = nimg_x; k.b = ((int64_t)g.H << 32) | (uint32_t)g.W; k.v[0] = g.Cin; k.v[7] = 3;
+        int rc = cached_map(&p.amap, k, [&](CUtensorMap* m) {
+            cuuint64_t dims[4] = {(cuuint64_t)g.Cin, (cuuint64_t)g.W, (cuuint64_t)g.H, (cuuint64_t)nimg_x};
+            cuuint64_t strides[3] = {(cuuint64_t)g.Cin * 4, (cuuint64_t)g.W * g.Cin * 4, (cuuint64_t)g.H * g.W * g.Cin * 4};
+            cuuint32_t box[4] = {32, 32, 1, 1}, estr[4] = {1, 1, 1, 1};
+            CUresult r = g_encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)x, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+            if (r != CUDA_SUCCESS) {
+                set_error("cuTensorMapEncodeTiled(wgrad x N=%ld H=%d W=%d C=%d) failed: %d", nimg_x, g.H, g.W, g.Cin, (int)r);
+                return (int)CG_ERR_CUDA;
+            }
+            return (int)CG_OK;
+        });
+        if (rc) return rc;
+    }
+    // channel-major copy of dy: (W, H, C, N), box (32 px, 1, BN channels, 1)
+    {
+        MapKey k{};
+        k.ptr = copy; k.a = nimg_dy; k.b = ((int64_t)g.Ho << 32) | (uint32_t)g.Wo; k.v[0] = g.Cout; k.v[1] = q.bn; k.v[7] = 4;
+        int rc = cached_map(&p.bmap, k, [&](CUtensorMap* m) {
+            cuuint64_t dims[4] = {(cuuint64_t)g.Wo, (cuuint64_t)g.Ho, (cuuint64_t)g.Cout, (cuuint64_t)nimg_dy};
+            cuuint64_t strides[3] = {(cuuint64_t)g.Wo * 4, (cuuint64_t)g.Ho * g.Wo * 4, (cuuint64_t)g.Cout * g.Ho * g.Wo * 4};
+            cuuint32_t box[4] = {32, 1, (cuuint32_t)q.bn, 1}, estr[4] = {1, 1, 1, 1};
+            CUresult r = g_encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)copy, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+            if (r != CUDA_SUCCESS) {
+                set_error("cuTensorMapEncodeTiled(wgrad dy copy N=%ld H=%d W=%d C=%d) failed: %d", nimg_dy, g.Ho, g.Wo, g.Cout, (int)r);
+                return (int)CG_ERR_CUDA;
+            }
+            return (int)CG_OK;
+        });
+        if (rc) return rc;
+    }
+    p.out = q.splits == 1 ? dw : part;
+    p.G = g.G; p.KW = g.KW; p.taps = g.KH * g.KW; p.M = g.Cin; p.N = g.Cout; p.Cin = g.Cin; p.Cout = g.Cout;
+    p.a_gimg = g.x_groups == 1 ? 0 : g.B;
+    p.b_gimg = g.B;
+    p.Hc = g.Ho; p.cpr = q.cpr; p.pad = g.pad;
+    p.chunks = q.chunks; p.split_chunks = q.split_chunks;
+    p.units = q.splits * g.G * p.taps * cdiv(g.Cin, q.bm) * cdiv(g.Cout, q.bn);
+    int rc;
+    if (q.bm == 64) rc = launch_wt<64, 64>(p, q.slots, st);
+    else if (q.bn == 64) rc = launch_wt<128, 64>(p, q.slots, st);
+    else if (q.bn == 128) rc = launch_wt<128, 128>(p, q.slots, st);
+    else rc = launch_wt<128, 256>(p, q.slots, st);
+    if (rc) return rc;
+    if (q.splits > 1) {
+        long n4 = (long)g.G * g.Cout * g.KH * g.KW * g.Cin / 4;
+        launch_k(reduce_splits_tc_kernel, cdiv(n4, 256), 256, 0, st, (const float*)part, dw, n4, q.splits);
+        return check_launch("reduce_splits_tc");
+    }
+    return CG_OK;
+}
+
 bool tc_wgrad_supported(const cg_conv_geom& g) {
+    if (tc_wgrad_tma_supported(g)) return true;
     if (g.ups) return false;
     if (g.Cin % 32 != 0 || g.Cout % 4 != 0) return false;
     long Mpix = (long)g.B * g.Ho * g.Wo;
@@ -874,6 +1214,10 @@ bool tc_wgrad_supported(const cg_conv_geom& g) {
 }
 
 size_t tc_wgrad_ws(const cg_conv_geom& g) {
+    if (tc_wgrad_tma_supported(g)) {
+        const WtPlan q = wt_plan(g);
+        return (size_t)(q.copy_bytes + q.part_bytes);
+    }
     int splits; long chunk;
     wg_plan(g, splits, chunk);
     if (splits == 1) return 0;
@@ -883,6 +1227,14 @@ size_t tc_wgrad_ws(const cg_conv_geom& g) {
 int tc_sm_count() { return sm_count_now(); }
 
 int tc_conv_wgrad(const cg_conv_geom& g, const float* x, const float* dy, float* dw, void* ws, size_t ws_bytes, cudaStream_t st) {
+    if (tc_wgrad_tma_supported(g)) {
+        size_t need = tc_wgrad_ws(g);
+        if (need > ws_bytes) {
+            set_error("conv_wgrad(tc, tma): workspace %zu < %zu bytes", ws_bytes, need);
+            return CG_ERR_WORKSPACE;
+        }
+        return tc_conv_wgrad_tma(g, x, dy, dw, ws, st);
+    }
     WgParams p{};
     int splits;
     wg_plan(g, splits, p.chunk);
