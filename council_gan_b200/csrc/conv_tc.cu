@@ -21,7 +21,7 @@
 // Kernels in this file (host dispatch at the bottom of each section):
 //   conv_tc_kernel<BK, BN>  forward / data gradient
 //   wgrad_tc_kernel<BM, BN> weight gradient (MN-major operands transposed in shared memory, then wgmma)
-//   wgrad_tma_kernel<BM, BN> weight gradient of stride-1 KxK layers (TMA-fed, shifted operand from registers)
+//   wgrad_tma_kernel<BM, BN> weight gradient of stride-1 and stride-2 KxK layers (TMA-fed, shifted operand from registers)
 //
 // Reference call sites replaced: nn.Conv2d forward (networks.py:513,516) and cuDNN dgrad via autograd.
 #include "common.cuh"
@@ -868,41 +868,47 @@ static void wg_plan(const cg_conv_geom& g, int& splits, long& chunk) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// weight gradient of stride-1 convolutions with KH*KW > 1: TMA-fed wgmma pipeline, shifted operand from registers
+// weight gradient of stride-1 and stride-2 convolutions with KH*KW > 1: TMA-fed wgmma pipeline, shifted operand from registers
 //
-// For tap k = (kh, kw) and stride 1,  dW[k][co][ci] = sum over x pixels p of dy[p - k + pad][co] * x[p][ci]
-//                                                    = sum over dy pixels o of x[o + k - pad][ci] * dy[o][co],
+// For tap k = (kh, kw) and stride s,  dW[k][co][ci] = sum over dy pixels o of x[s o + k - pad][ci] * dy[o][co],
 // out-of-range x pixels counting as zero.  The reduction (K) runs over dy pixels, x is read at tap-shifted pixels.
+// * Writing k - pad = s a + r with 0 <= r < s (per axis), x row s oh + k - pad is row oh + a of the row-parity-r sub-grid of x:
+//   in a parity view of x every tap is a whole-pixel shift a of the dy grid.  The view is a 5-D tiled map over the unchanged
+//   channels-last memory, (s Cin, W / s, s, H / s, N): the column parity is folded into the channel coordinate (r_w Cin + ci), the
+//   row parity is its own coordinate.  For s = 1 it is the plain (C, W, 1, H, N) view.
 // * dy is "copied": a transpose kernel writes it channel-major [img][Cout][Ho][Wo], TF32-rounded, into the workspace once per
-//   call, and a 4-D tiled map (W, H, C, N) with a (32 px, 1, BN channels, 1) box brings 32 pixels of one row straight into the
-//   K-major 128-byte-swizzled layout wgmma reads as its B operand.  Chunk starts are multiples of 32 pixels, so the innermost
-//   TMA coordinate stays aligned; a partial last chunk of a row is zero-filled.
-// * x ("direct") is read from its channels-last layout with a (C, W, H, N) map, box (32 channels, 32 px, 1, 1): the tap shift
-//   moves the W and H coordinates, which are outer dimensions, so starts off the map are legal and zero-filled (the padding).
+//   call, and a 4-D tiled map with a (32 px, 1, BN channels, 1) box brings 32 pixels straight into the K-major
+//   128-byte-swizzled layout wgmma reads as its B operand.  Where Wo >= 32 the map is (Wo, Ho, C, N) and a chunk is 32 pixels of
+//   one row; chunk starts are multiples of 32 pixels, so the innermost TMA coordinate stays aligned, and a partial last chunk of
+//   a row is zero-filled.  Where Wo < 32 divides 32 (and 32 divides Ho Wo) a chunk is 32 / Wo whole rows, and the same memory
+//   is mapped as (32, Ho Wo / 32, C, N).
+// * x ("direct") is read through the parity view, box (32 channels, 32 px, 1, 1, 1), or (32 channels, Wo px, 1, 32 / Wo rows, 1)
+//   for whole-row chunks; both land as [pixel][32 channels] in the chunk's pixel order.  The tap shift moves the W / s and H / s
+//   coordinates, which are outer dimensions, so starts off the map are legal and zero-filled (the padding).
 //   That tile is MN-major, which wgmma cannot take as a TF32 shared-memory operand; the consumers read their A fragments out of
 //   it with LDS, round them to TF32 and issue the register-A ("RS") form of wgmma.
 // * M = Cin, N = Cout: the epilogue stores D transposed into dw[g][co][kh][kw][ci].
 // * Same arithmetic as wgrad_tc_kernel: the same TF32-rounded operands, the same pixel splits (wg_plan), and within a split the
-//   same 8-pixel k-steps in the same order, so where Wo % 32 == 0 (a 32-pixel chunk of dy is 32 consecutive pixels of one row)
-//   both kernels produce the same bits.  Training amplifies any rounding difference in the weight gradients within a few steps,
-//   so a kernel that merely agreed to rounding would change what a training run computes.
+//   same 8-pixel k-steps in the same order, so where a 32-pixel chunk is 32 consecutive pixels of dy (Wo % 32 == 0, or whole-row
+//   chunks) both kernels produce the same bits.  Training amplifies any rounding difference in the weight gradients within a
+//   few steps, so a kernel that merely agreed to rounding would change what a training run computes.
 // * Warp-specialised persistent CTAs as in conv_tc_kernel: one TMA producer thread, BM / 64 consumer warpgroups, a full / empty
 //   mbarrier ring.  Work units (pixel split, group, tap, M tile, N tile) are walked split-major, so that the CTAs running at the
 //   same time read the same pixel range and the KH*KW re-reads of it come from L2.  Splits write partials that
 //   reduce_splits_tc_kernel sums in a fixed order (deterministic).
 // ------------------------------------------------------------------------------------------------
-thread_local int g_wgrad_tma = 1;  // mode bit 25 clears it: stride-1 weight gradients stay on wgrad_tc_kernel
+thread_local int g_wgrad_tma = 1;  // mode bit 25 clears it: every layer this kernel serves stays on wgrad_tc_kernel
 
 constexpr int WT_MAX_STAGES = 8;
 
 struct WtParams {
-    CUtensorMap amap;               // x, channels-last
+    CUtensorMap amap;               // parity view of x, channels-last
     CUtensorMap bmap;               // channel-major copy of dy
     float* out;                     // [split][G][Cout][KH][KW][Cin]
     int G, KW, taps, M, N, Cin, Cout;
     int a_gimg, b_gimg;             // images per group in the x / dy-copy map (0: input shared by the council)
-    int Hc, cpr;                    // dy grid: rows per image, 32-pixel chunks per row
-    int pad;                        // x pixel = dy pixel + tap - pad
+    int Hc, cpr, rows;              // per image: chunk rows, 32-pixel chunks per chunk row; dy rows per chunk row
+    int pad, s_log2;                // x pixel = stride * dy pixel + tap - pad, stride = 1 << s_log2
     long chunks, split_chunks;      // chunks per member, per split
     int units, stages;
 };
@@ -960,7 +966,9 @@ __global__ void __launch_bounds__(2 * BM + 128, BM == 64 ? 2 : 1) wgrad_tma_kern
                 r /= p.taps;
                 const int g = r % p.G, split = r / p.G;
                 const int kh = tap / p.KW, kw = tap - kh * p.KW;
-                const int sh = kh - p.pad, sw = kw - p.pad;
+                // tap offset = stride * a + r per axis, 0 <= r < stride (arithmetic shift: floor division by a power of two)
+                const int ah = (kh - p.pad) >> p.s_log2, rh = kh - p.pad - (ah << p.s_log2);
+                const int aw = (kw - p.pad) >> p.s_log2, rw = kw - p.pad - (aw << p.s_log2);
                 int nbox = (p.M - m0) / 32;                // whole 32-channel boxes inside the tensor (M % 32 == 0)
                 if (nbox > BM / 32) nbox = BM / 32;       // rows past M are never stored: their boxes are not loaded
                 const uint32_t tx = (uint32_t)(nbox * A_BOX + BN * 128);
@@ -976,7 +984,8 @@ __global__ void __launch_bounds__(2 * BM + 128, BM == 64 ? 2 : 1) wgrad_tma_kern
                     mbar_expect_tx(&full_bar[stage], tx);
                     const int w0 = wq * 32;
                     for (int j = 0; j < nbox; j++)
-                        tma_load_4d(&p.amap, &full_bar[stage], sa + j * A_BOX, m0 + 32 * j, w0 + sw, h + sh, g * p.a_gimg + img);
+                        tma_load_5d(&p.amap, &full_bar[stage], sa + j * A_BOX, rw * p.Cin + m0 + 32 * j, w0 + aw, rh, h * p.rows + ah,
+                                    g * p.a_gimg + img);
                     tma_load_4d(&p.bmap, &full_bar[stage], sa + BM * 128, w0, h, n0, g * p.b_gimg + img);
                     if (++wq == p.cpr) { wq = 0; if (++h == p.Hc) { h = 0; ++img; } }
                     if (++stage == p.stages) { stage = 0; phase ^= 1; }
@@ -1084,33 +1093,43 @@ __global__ void __launch_bounds__(256) nhwc_to_nchw_tf32_kernel(const float* __r
     }
 }
 
+// dy rows per 32-pixel chunk: 32 / Wo whole rows where Wo < 32 divides 32 and the chunks tile each image, else 1
+static int wt_rows(const cg_conv_geom& g) { return g.Wo < 32 && 32 % g.Wo == 0 && g.Ho * g.Wo % 32 == 0 ? 32 / g.Wo : 1; }
+
 bool tc_wgrad_tma_supported(const cg_conv_geom& g) {
-    if (!g_wgrad_tma || g.stride != 1 || g.ups || g.KH * g.KW <= 1) return false;
+    if (!g_wgrad_tma || g.ups || g.KH * g.KW <= 1) return false;
+    if (g.stride != 1 && g.stride != 2) return false;
+    if (g.H % g.stride || g.W % g.stride) return false;  // the parity view of x is made of whole stride x stride cells
     if (g.Cin % 32 != 0 || g.Cout % 32 != 0) return false;
     init_driver();
     if (!g_encode_tiled) return false;
-    if (g.W < 32 || g.Wo < 32 || g.Wo % 4 != 0) return false;  // Wo % 4: TMA strides of the copy are multiples of 16 bytes
-    return (long)g.B * g.Ho * g.Wo >= 256;
+    if ((long)g.B * g.Ho * g.Wo < 256) return false;
+    const int rows = wt_rows(g), Hs = g.H / g.stride, Ws = g.W / g.stride;  // x box: 32 pixels of one row, or `rows` rows of Wo
+    if (rows > 1) return Ws >= g.Wo && Hs >= rows;
+    return Ws >= 32 && g.Wo >= 32 && g.Wo % 4 == 0;  // Wo % 4: TMA strides of the copy are multiples of 16 bytes
 }
 
 struct WtPlan {
-    int bm, bn, cpr, splits, slots;
+    int bm, bn, rows, cpr, splits, slots;
     long chunks, split_chunks, copy_bytes, part_bytes;
 };
 
 static WtPlan wt_plan(const cg_conv_geom& g) {
     WtPlan q;
+    // one consumer warpgroup (BM = 64) where Cin <= 64; 64 x 128 tiles there read each x chunk once for 128 output channels,
+    // 1.5x the rate of 64 x 64 tiles on the 4x4 64->128 layers
     q.bm = g.Cin > 64 ? 128 : 64;
-    q.bn = q.bm == 64 ? 64 : g.Cout >= 256 ? 256 : g.Cout > 64 ? 128 : 64;
-    q.cpr = cdiv(g.Wo, 32);
-    q.chunks = (long)g.B * g.Ho * q.cpr;
+    q.bn = q.bm == 128 && g.Cout >= 256 ? 256 : g.Cout > 64 ? 128 : 64;
+    q.rows = wt_rows(g);
+    q.cpr = q.rows > 1 ? 1 : cdiv(g.Wo, 32);
+    q.chunks = (long)g.B * (g.Ho / q.rows) * q.cpr;
     q.copy_bytes = (((long)g.G * g.B * g.Ho * g.Wo * g.Cout * 4) + 1023) & ~1023L;
-    q.slots = (q.bm == 64 ? 2 : 1) * sm_count_now();  // two CTAs per SM for the single-warpgroup 64 x 64 tiles
+    q.slots = (q.bm == 64 ? 2 : 1) * sm_count_now();  // two CTAs per SM for the single-warpgroup tiles
     // the pixel splits of wgrad_tc_kernel (see the section comment); `chunk` is a multiple of 32 pixels
     int splits;
     long chunk;
     wg_plan(g, splits, chunk);
-    q.split_chunks = g.Wo % 32 == 0 ? chunk / 32 : (q.chunks + splits - 1) / splits;
+    q.split_chunks = g.Wo % 32 == 0 || q.rows > 1 ? chunk / 32 : (q.chunks + splits - 1) / splits;
     q.splits = (int)((q.chunks + q.split_chunks - 1) / q.split_chunks);
     q.part_bytes = q.splits > 1 ? (long)q.splits * g.G * g.Cout * g.KH * g.KW * g.Cin * 4 : 0;
     return q;
@@ -1119,7 +1138,7 @@ static WtPlan wt_plan(const cg_conv_geom& g) {
 template <int BM, int BN>
 static int launch_wt(WtParams& p, int slots, cudaStream_t st) {
     constexpr int STAGE = (BM + BN) * 128;
-    // 64 x 64 tiles: two CTAs per SM (228 KB of shared memory per SM, 1 KB of it reserved per CTA)
+    // BM = 64: two CTAs per SM (228 KB of shared memory per SM, 1 KB of it reserved per CTA)
     int stages = ((BM == 64 ? 110 : 225) * 1024 - 1024 - 2 * WT_MAX_STAGES * 8) / STAGE;
     if (stages > WT_MAX_STAGES) stages = WT_MAX_STAGES;
     p.stages = stages;
@@ -1143,36 +1162,43 @@ static int tc_conv_wgrad_tma(const cg_conv_geom& g, const float* x, const float*
     float* copy = (float*)ws;
     float* part = (float*)((uint8_t*)ws + q.copy_bytes);
     const long nimg_x = g.x_groups == 1 ? g.B : (long)g.G * g.B, nimg_dy = (long)g.G * g.B;
-    launch_k(nhwc_to_nchw_tf32_kernel, dim3(q.cpr * (g.Cout / 32), g.Ho, (unsigned)nimg_dy), 256, 0, st, dy, copy, g.Ho, g.Wo, g.Cout);
+    launch_k(nhwc_to_nchw_tf32_kernel, dim3(cdiv(g.Wo, 32) * (g.Cout / 32), g.Ho, (unsigned)nimg_dy), 256, 0, st, dy, copy, g.Ho, g.Wo,
+             g.Cout);
     if (int rc = check_launch("nhwc_to_nchw_tf32")) return rc;
 
     // Both maps move raw fp32 (the copy is already rounded, x is rounded in registers), whatever a TF32 map would do to the low bits.
     WtParams p{};
-    // x: channels-last (C, W, H, N), box (32 channels, 32 px, 1, 1)
+    // x: parity view (s C, W / s, s, H / s, N) of the channels-last tensor, box (32 channels, 32 px, 1, 1, 1) or
+    // (32 channels, Wo px, 1, rows, 1)
     {
+        const int s = g.stride, box_w = q.rows > 1 ? g.Wo : 32;
         MapKey k{};
-        k.ptr = x; k.a = nimg_x; k.b = ((int64_t)g.H << 32) | (uint32_t)g.W; k.v[0] = g.Cin; k.v[7] = 3;
+        k.ptr = x; k.a = nimg_x; k.b = ((int64_t)g.H << 32) | (uint32_t)g.W;
+        k.v[0] = g.Cin; k.v[1] = s; k.v[2] = box_w; k.v[3] = q.rows; k.v[7] = 3;
         int rc = cached_map(&p.amap, k, [&](CUtensorMap* m) {
-            cuuint64_t dims[4] = {(cuuint64_t)g.Cin, (cuuint64_t)g.W, (cuuint64_t)g.H, (cuuint64_t)nimg_x};
-            cuuint64_t strides[3] = {(cuuint64_t)g.Cin * 4, (cuuint64_t)g.W * g.Cin * 4, (cuuint64_t)g.H * g.W * g.Cin * 4};
-            cuuint32_t box[4] = {32, 32, 1, 1}, estr[4] = {1, 1, 1, 1};
-            CUresult r = g_encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)x, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+            cuuint64_t dims[5] = {(cuuint64_t)s * g.Cin, (cuuint64_t)(g.W / s), (cuuint64_t)s, (cuuint64_t)(g.H / s), (cuuint64_t)nimg_x};
+            cuuint64_t strides[4] = {(cuuint64_t)s * g.Cin * 4, (cuuint64_t)g.W * g.Cin * 4, (cuuint64_t)s * g.W * g.Cin * 4,
+                                     (cuuint64_t)g.H * g.W * g.Cin * 4};
+            cuuint32_t box[5] = {32, (cuuint32_t)box_w, 1, (cuuint32_t)q.rows, 1}, estr[5] = {1, 1, 1, 1, 1};
+            CUresult r = g_encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, (void*)x, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
             if (r != CUDA_SUCCESS) {
-                set_error("cuTensorMapEncodeTiled(wgrad x N=%ld H=%d W=%d C=%d) failed: %d", nimg_x, g.H, g.W, g.Cin, (int)r);
+                set_error("cuTensorMapEncodeTiled(wgrad x N=%ld H=%d W=%d C=%d stride %d box %dx%d) failed: %d", nimg_x, g.H, g.W, g.Cin, s,
+                          q.rows, box_w, (int)r);
                 return (int)CG_ERR_CUDA;
             }
             return (int)CG_OK;
         });
         if (rc) return rc;
     }
-    // channel-major copy of dy: (W, H, C, N), box (32 px, 1, BN channels, 1)
+    // channel-major copy of dy: (Wo, Ho, C, N), or (32, Ho Wo / 32, C, N) for whole-row chunks; box (32 px, 1, BN channels, 1)
     {
+        const int cw = q.rows > 1 ? 32 : g.Wo;
         MapKey k{};
         k.ptr = copy; k.a = nimg_dy; k.b = ((int64_t)g.Ho << 32) | (uint32_t)g.Wo; k.v[0] = g.Cout; k.v[1] = q.bn; k.v[7] = 4;
         int rc = cached_map(&p.bmap, k, [&](CUtensorMap* m) {
-            cuuint64_t dims[4] = {(cuuint64_t)g.Wo, (cuuint64_t)g.Ho, (cuuint64_t)g.Cout, (cuuint64_t)nimg_dy};
-            cuuint64_t strides[3] = {(cuuint64_t)g.Wo * 4, (cuuint64_t)g.Ho * g.Wo * 4, (cuuint64_t)g.Cout * g.Ho * g.Wo * 4};
+            cuuint64_t dims[4] = {(cuuint64_t)cw, (cuuint64_t)g.Ho * g.Wo / cw, (cuuint64_t)g.Cout, (cuuint64_t)nimg_dy};
+            cuuint64_t strides[3] = {(cuuint64_t)cw * 4, (cuuint64_t)g.Ho * g.Wo * 4, (cuuint64_t)g.Cout * g.Ho * g.Wo * 4};
             cuuint32_t box[4] = {32, 1, (cuuint32_t)q.bn, 1}, estr[4] = {1, 1, 1, 1};
             CUresult r = g_encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)copy, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -1188,11 +1214,12 @@ static int tc_conv_wgrad_tma(const cg_conv_geom& g, const float* x, const float*
     p.G = g.G; p.KW = g.KW; p.taps = g.KH * g.KW; p.M = g.Cin; p.N = g.Cout; p.Cin = g.Cin; p.Cout = g.Cout;
     p.a_gimg = g.x_groups == 1 ? 0 : g.B;
     p.b_gimg = g.B;
-    p.Hc = g.Ho; p.cpr = q.cpr; p.pad = g.pad;
+    p.Hc = g.Ho / q.rows; p.cpr = q.cpr; p.rows = q.rows;
+    p.pad = g.pad; p.s_log2 = g.stride == 2;
     p.chunks = q.chunks; p.split_chunks = q.split_chunks;
     p.units = q.splits * g.G * p.taps * cdiv(g.Cin, q.bm) * cdiv(g.Cout, q.bn);
     int rc;
-    if (q.bm == 64) rc = launch_wt<64, 64>(p, q.slots, st);
+    if (q.bm == 64) rc = q.bn == 64 ? launch_wt<64, 64>(p, q.slots, st) : launch_wt<64, 128>(p, q.slots, st);
     else if (q.bn == 64) rc = launch_wt<128, 64>(p, q.slots, st);
     else if (q.bn == 128) rc = launch_wt<128, 128>(p, q.slots, st);
     else rc = launch_wt<128, 256>(p, q.slots, st);

@@ -59,9 +59,9 @@ int cg_device_info(int* sm_count, int* cc_major, int* cc_minor);
  * (internally 1 forward | 2 dgrad | 4 wgrad).  Switches on top of the mask: 1<<22 = programmatic dependent launch between this
  * library's kernels (every kernel carries the griddepcontrol pair; the trainer turns it on for small maps only), 1<<24 = programmatic
  * dependent launch for the helper kernels only (those without dynamic shared memory), 1<<23 = keep the widest N tile on small maps
- * (default: narrower tiles when a launch has fewer tiles than SMs), 1<<25 = weight gradients of stride-1 KxK layers on the
- * previous tensor-core kernel, which transposes both operands in the MMA warps, for comparisons in one process (default: the
- * TMA-fed kernel that reads one operand from a channel-major copy).  Other bits are accepted and ignored.
+ * (default: narrower tiles when a launch has fewer tiles than SMs), 1<<25 = weight gradients of stride-1 and stride-2 KxK layers
+ * on the previous tensor-core kernel, which transposes both operands in the MMA warps, for comparisons in one process (default:
+ * the TMA-fed kernel that reads one operand from a channel-major copy).  Other bits are accepted and ignored.
  * The switches are per calling thread (like cg_last_error), not process-global.  Returns the previous mask. */
 int cg_set_tensor_core_mode(int mode);
 /* number of kernels launched by this library since load (bench.py reports it as gpu_launches) */
