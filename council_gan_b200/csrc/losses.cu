@@ -9,6 +9,8 @@
 //   mask_zero_one_criterion / mask_small_criterion(_square) / mask_criterion_TV   trainer_council.py:230-250
 //   loss-history matching                                   trainer_council.py:518-524, 576-586
 //   total-loss assembly in gen_update                       trainer_council.py:392-451, 497-529, 559-634
+//   abs_beginning_end (recon_criterion_v2_color)            trainer_council.py:210-215, 477-495  (2 more launches per direction
+//                                                           while its weight gate is open)
 #include "common.cuh"
 
 namespace cg {
@@ -322,6 +324,90 @@ __global__ void __launch_bounds__(256) gen_loss_bwd_kernel(const cg_gen_loss_des
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// gen_update, abs_beginning_end: recon_criterion_v2_color(x_fake, x) (trainer_council.py:210-215, 477-495), d = x_fake - x
+// over the 3 live lanes; L1 = mean |d|, L2 = mean d^2, the loss is L1 if L1 > L2 else L2
+// ---------------------------------------------------------------------------------------------------------------
+// pass 1: block (chunk, g) sums |d| and d^2 over GL_PIX pixels in float, the last block adds the chunks in double (the
+// convention of the focus sums).  part: float [nchunks][G][2].
+__global__ void __launch_bounds__(256) abs_be_fwd_kernel(const float* __restrict__ x_fake, const float* __restrict__ x, float* __restrict__ sums,
+                                                         float* __restrict__ part, unsigned int* __restrict__ counter, int G, long npix,
+                                                         int nchunks) {
+    pdl_trigger();
+    pdl_wait();
+    __shared__ float sm[2 * 32];
+    const int g = blockIdx.x % G, chunk = blockIdx.x / G;
+    const long p0 = (long)chunk * GL_PIX, p1 = min(npix, p0 + GL_PIX);
+    const float* xf = x_fake + (long)g * npix * 4;
+    float v[2] = {0.f, 0.f};
+    for (long px = p0 + threadIdx.x; px < p1; px += blockDim.x) {
+        const float4 a = ld4(xf + px * 4), b = ld4(x + px * 4);
+        const float d0 = a.x - b.x, d1 = a.y - b.y, d2 = a.z - b.z;
+        v[0] += fabsf(d0) + fabsf(d1) + fabsf(d2);
+        v[1] += d0 * d0 + d1 * d1 + d2 * d2;
+    }
+    block_sum<2>(v, sm);
+    if (threadIdx.x == 0) {
+        float* o = part + ((long)chunk * G + g) * 2;
+        o[0] = v[0]; o[1] = v[1];
+    }
+    if (!last_block_done(counter, gridDim.x)) return;
+    const int t = threadIdx.x;  // sums[g][k] = sum over chunks of part[c][g][k], k = 0 (|d|), 1 (d^2)
+    if (t < G * 2) {
+        const volatile float* vp = part;
+        double s = 0.0;
+        for (int c = 0; c < nchunks; c++) s += (double)vp[(long)c * G * 2 + t];
+        sums[t] = (float)s;
+    }
+    if (t == 0) *counter = 0u;
+}
+
+struct AbsBeWeights { double w[CG_LOSS_MAX_G]; };  // per member; 0: no contribution (the member's gate is closed)
+
+// pass 2 (sums summed over ranks): every block derives the branch and the gradient coefficient of each member; block 0 publishes
+// the unweighted loss and adds w * loss to the double accumulator of the direction totals (the one cg_gen_loss_bwd keeps in the
+// same workspace); then a grid-stride pass adds the gradient to d_x: w/numel * sign(d) (L1; sign(0) = 0) or w/numel * 2d (L2).
+__global__ void __launch_bounds__(256) abs_be_bwd_kernel(const float* __restrict__ x_fake, const float* __restrict__ x, const float* __restrict__ sums,
+                                                         double numel, const AbsBeWeights wt, int G, long npix, float* __restrict__ total,
+                                                         double* __restrict__ total64, float* __restrict__ pub, float* __restrict__ d_x) {
+    pdl_trigger();
+    pdl_wait();
+    __shared__ float s_coef[CG_LOSS_MAX_G];
+    __shared__ int s_l1[CG_LOSS_MAX_G];
+    if (threadIdx.x < G) {
+        const int g = threadIdx.x;
+        const double l1 = (double)sums[2 * g] / numel, l2 = (double)sums[2 * g + 1] / numel;
+        const bool use_l1 = l1 > l2;  // a tie picks L2
+        const double val = use_l1 ? l1 : l2, w = wt.w[g];
+        s_l1[g] = use_l1;
+        s_coef[g] = (float)((use_l1 ? 1.0 : 2.0) * w / numel);
+        if (blockIdx.x == 0) {
+            pub[g] = (float)val;
+            if (w != 0.0) {
+                const double t64 = total64[g] + w * val;
+                total64[g] = t64;
+                total[g] = (float)t64;
+            }
+        }
+    }
+    __syncthreads();
+    const long total_px = npix * G, stride = (long)gridDim.x * blockDim.x;
+    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total_px; i += stride) {
+        const int g = (int)(i / npix);
+        const float c = s_coef[g];
+        if (c == 0.f) continue;
+        const float4 a = ld4(x_fake + i * 4), b = ld4(x + (i - (long)g * npix) * 4);
+        const float d0 = a.x - b.x, d1 = a.y - b.y, d2 = a.z - b.z;
+        float4 o = reinterpret_cast<const float4*>(d_x)[i];
+        if (s_l1[g]) {
+            o.x += c * sgnf(d0); o.y += c * sgnf(d1); o.z += c * sgnf(d2);
+        } else {
+            o.x += c * d0; o.y += c * d1; o.z += c * d2;
+        }
+        reinterpret_cast<float4*>(d_x)[i] = o;
+    }
+}
+
 }  // namespace cg
 
 using namespace cg;
@@ -406,4 +492,36 @@ extern "C" int cg_gen_loss_bwd(const cg_gen_loss_desc* d, const cg_gen_loss_hp* 
     launch_k(gen_loss_bwd_kernel, blocks, 256, 0, ST, *d, *hp, scal, hist_gan, hist_council, total, ws_total64(ws), accumulate, pub, d_mask,
                                                 map_blocks);
     return check_launch("gen_loss_bwd");
+}
+
+extern "C" int cg_abs_beginning_end_fwd(const float* x_fake, const float* x, float* sums, int G, int B, int H, int W, void* ws,
+                                        size_t ws_bytes, void* stream) {
+    CG_REQUIRE(x_fake && x && sums && G >= 1 && G <= CG_LOSS_MAX_G && B >= 1 && H >= 1 && W >= 1,
+               "abs_beginning_end_fwd: G=%d B=%d H=%d W=%d out of range", G, B, H, W);
+    const long npix = (long)B * H * W;
+    const int nchunks = cdiv(npix, GL_PIX);
+    size_t need = 16 + CG_LOSS_MAX_G * 8 + (size_t)nchunks * G * 2 * 4;
+    if (need > ws_bytes) {
+        set_error("abs_beginning_end_fwd: workspace %zu < %zu bytes", ws_bytes, need);
+        return CG_ERR_WORKSPACE;
+    }
+    launch_k(abs_be_fwd_kernel, nchunks * G, 256, 0, ST, x_fake, x, sums, ws_part(ws), ws_counter(ws), G, npix, nchunks);
+    return check_launch("abs_beginning_end_fwd");
+}
+
+extern "C" int cg_abs_beginning_end_bwd(const float* x_fake, const float* x, const float* sums, double numel, const double* host_weight,
+                                        float* total, float* pub, float* d_x, int G, int B, int H, int W, void* ws, size_t ws_bytes,
+                                        void* stream) {
+    CG_REQUIRE(x_fake && x && sums && host_weight && total && pub && d_x && G >= 1 && G <= CG_LOSS_MAX_G && B >= 1 && H >= 1 && W >= 1,
+               "abs_beginning_end_bwd: G=%d B=%d H=%d W=%d out of range", G, B, H, W);
+    CG_REQUIRE(numel > 0, "abs_beginning_end_bwd: numel must be positive");
+    CG_REQUIRE(ws_bytes >= 16 + CG_LOSS_MAX_G * 8, "abs_beginning_end_bwd: workspace too small");
+    AbsBeWeights wt = {};
+    for (int g = 0; g < G; g++) wt.w[g] = host_weight[g];
+    const long npix = (long)B * H * W;
+    int blocks = cdiv(npix * G, 256);
+    const int cap = 8 * (tc_sm_count() > 0 ? tc_sm_count() : 1);
+    if (blocks > cap) blocks = cap;
+    launch_k(abs_be_bwd_kernel, blocks, 256, 0, ST, x_fake, x, sums, numel, wt, G, npix, total, ws_total64(ws), pub, d_x);
+    return check_launch("abs_beginning_end_bwd");
 }

@@ -84,6 +84,9 @@ _SIGS = {
     'cg_lsgan_fused': (C.c_int, [C.POINTER(LsganDesc), _fp, C.c_int, _fp, _fp, C.c_size_t, _fp]),
     'cg_gen_loss_fwd': (C.c_int, [C.POINTER(GenLossDesc), _fp, _fp, C.c_size_t, _fp]),
     'cg_gen_loss_bwd': (C.c_int, [C.POINTER(GenLossDesc), C.POINTER(GenLossHp), _fp, _fp, _fp, _fp, C.c_int, _fp, _fp, _fp, C.c_size_t, _fp]),
+    'cg_abs_beginning_end_fwd': (C.c_int, [_fp, _fp, _fp] + [C.c_int] * 4 + [_fp, C.c_size_t, _fp]),
+    'cg_abs_beginning_end_bwd': (C.c_int, [_fp, _fp, _fp, C.c_double, C.POINTER(C.c_double), _fp, _fp, _fp] + [C.c_int] * 4 +
+                                 [_fp, C.c_size_t, _fp]),
     'cg_loss_workspace_bytes': (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int]),
     'cg_zero': (C.c_int, [_fp, C.c_size_t, _fp]),
     'cg_aug_color': (C.c_int, [_fp, _fp, _fp, _fp, _fp, C.c_int, C.c_int, C.c_int, _fp]),
@@ -628,6 +631,28 @@ class CudaOps:
                                           int(bool(accumulate)), _p(pub), _p(d_mask), _p(ws), ws.numel(), self._stream()),
                  'cg_gen_loss_bwd')
         return cl_douts, d_mask
+
+    def abs_beginning_end_fwd(self, x_fake, x, sums):
+        """Pass 1 of abs_beginning_end: sums[G,2] = {sum |x_fake - x|, sum (x_fake - x)^2} over the 3 live lanes of this rank.
+        x_fake [G,B,H,W,4], x [1,B,H,W,4] (shared).  ONE launch."""
+        self._chk(x_fake, x, sums)
+        G, B, H, W, _ = x_fake.shape
+        assert tuple(x.shape) == (1, B, H, W, 4) and sums.numel() == 2 * G
+        ws = self._loss_scratch(G, B, H, W)
+        self._ck(self.lib.cg_abs_beginning_end_fwd(_p(x_fake), _p(x), _p(sums), G, B, H, W, _p(ws), ws.numel(), self._stream()),
+                 'cg_abs_beginning_end_fwd')
+
+    def abs_beginning_end_bwd(self, x_fake, x, sums, numel, weights, total, pub, d_x):
+        """Pass 2: picks L1 or L2 per member from the (globally summed) sums, pub[g] = the unweighted loss, total[g] += weights[g] *
+        loss, d_x += its gradient.  weights: python floats, 0 = no contribution.  Must follow gen_loss_bwd of the same direction
+        (the direction totals share its double accumulator).  ONE launch."""
+        self._chk(x_fake, x, sums, total, pub, d_x)
+        G, B, H, W, _ = x_fake.shape
+        assert tuple(d_x.shape) == tuple(x_fake.shape) and len(weights) == G
+        w = (C.c_double * G)(*weights)
+        ws = self._loss_scratch(G)  # never grows the scratch: a new buffer would drop the accumulator gen_loss_bwd left in it
+        self._ck(self.lib.cg_abs_beginning_end_bwd(_p(x_fake), _p(x), _p(sums), float(numel), w, _p(total), _p(pub), _p(d_x), G, B, H, W,
+                                                   _p(ws), ws.numel(), self._stream()), 'cg_abs_beginning_end_bwd')
 
     # -- input pipeline (council_gan_b200/data.py) ------------------------------------------------------
     def aug_color(self, pix, desc, opcode, param, B, max_pixels, any_contrast):

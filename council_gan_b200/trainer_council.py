@@ -24,7 +24,11 @@ What is different underneath (GPU-first, see DESIGN.md):
     once per optimiser step -- asynchronously: the discriminators' all-reduce + Adam are joined only when that
     family's parameters are next needed (dis: during dis_council_update; dis_council: during gen_update's
     generator forward; gen: decoder bucket during the encoder backward).
-Paths outside the live configuration space of the reference's three configs (recon_*/vgg/abs losses,
+  * abs_beginning_end (:477-495, the input-to-output pixel loss whose weight decays with ``iterations``): its gate and
+    weight are host arithmetic on Python floats (``abs_beginning_end_w_conf``, with the reference's member-0 quirk); its value,
+    branch (L1 or L2) and gradient are two more launches per direction (csrc/losses.cu) whose sums join the scalar all-reduce.
+    With ``abs_beginning_end: 0`` (the shipped configs) nothing of it runs.
+Paths outside the live configuration space of the reference's three configs (recon_*/vgg/council_abs losses,
 nsgan/RaHinge, do_my_style, gray-scale D, random D/G pairing) raise NotImplementedError.
 """
 from __future__ import annotations
@@ -216,8 +220,7 @@ class Council_Trainer(nn.Module):
     # ------------------------------------------------------------------------------------------------
     @staticmethod
     def _check_supported(hp):
-        bad = [k for k in ('recon_x_w', 'recon_s_w', 'recon_c_w', 'recon_x_cyc_w', 'vgg_w', 'abs_beginning_end',
-                           'council_abs_w') if hp.get(k, 0) != 0]
+        bad = [k for k in ('recon_x_w', 'recon_s_w', 'recon_c_w', 'recon_x_cyc_w', 'vgg_w', 'council_abs_w') if hp.get(k, 0) != 0]
         if bad:
             raise NotImplementedError('loss terms %s are not on the accelerated training path' % bad)
         if hp['dis']['gan_type'] != 'lsgan':
@@ -261,6 +264,23 @@ class Council_Trainer(nn.Module):
         if for_gen and hp['iteration'] < c['council_start_at_iter']:
             do = False
         return do
+
+    def _abs_beginning_end_weights(self, hp, iterations):
+        """Gate and weight of the abs_beginning_end term, trainer_council.py:477-495, on host floats.  Member i gets the term while
+        abs_beginning_end != 0 and abs_beginning_end_w_conf > 0.005; the weight is recomputed inside the member loop, so member 0 is
+        gated by the previous call's weight and the others by this call's.  Once the weight is at or below 0.005 the block is never
+        entered again and the weight stops updating.  -> None when the term is off, else the weights of the members whose gate
+        is open (a prefix of the council, possibly empty)."""
+        if hp['abs_beginning_end'] == 0:
+            return None
+        weights = []
+        for _ in range(self.council_size):
+            if not self.abs_beginning_end_w_conf > 0.005:
+                break
+            self.abs_beginning_end_w_conf = max(hp['abs_beginning_end'] * hp['abs_beginning_end_less_by'] ** iterations,
+                                                hp['abs_beginning_end_minimume'])
+            weights.append(self.abs_beginning_end_w_conf)
+        return weights
 
     # ---- small host/device helpers ---------------------------------------------------------------------
     def _img(self, x):
@@ -535,10 +555,17 @@ class Council_Trainer(nn.Module):
         council_on = (hp['council_w'] != 0) and self.do_council_loss and N > 1 and self.do_dis_council  # :559,567
         gan_on = hp['gan_w'] != 0
         center, eps = float(fl['mask_zero_or_one_center']), float(fl['mask_zero_or_one_epsilon'])
+        be_w = self._abs_beginning_end_weights(hp, iterations)
+        be_on = bool(be_w)
 
         # ---- forward of every direction; pass 1 of the loss (all reductions, one launch per direction) -----------
         fw = {}
-        scal = ops.empty(len(self._dirs), N, 6)  # per direction and member: [adv, council, focus sums x4] of THIS rank
+        nd = len(self._dirs)
+        if be_on:  # the abs_beginning_end sums [|d|, d^2] ride behind the other scalars: still one all-reduce
+            red = ops.empty(nd * N * 8)
+            scal, be_sums = red[:nd * N * 6].view(nd, N, 6), red[nd * N * 6:].view(nd, N, 2)
+        else:
+            red = scal = ops.empty(nd, N, 6)  # per direction and member: [adv, council, focus sums x4] of THIS rank
         for di, d in enumerate(self._dirs):
             gen = self._nets['gen_' + d]
             src = self._src(d, img_a, img_b)
@@ -562,15 +589,20 @@ class Council_Trainer(nn.Module):
                 rec['disc_outs'] = self._nets['dis_council_' + d].forward(xin, rec['disc_saved'])
             rec['d_adv'] = ops.gen_loss_fwd(rec['dis_outs'], rec['disc_outs'], mask if focus_on else None, center, eps,
                                             float(hp['gan_w']) / self.world, scal[di])
+            if be_on:
+                ops.abs_beginning_end_fwd(x_fake, src, be_sums[di])
             fw[d] = rec
         self._flush()  # (a family gated off above still steps here)
         dist = _dist()
         if dist is not None and self.world > 1:
-            dist.all_reduce(scal)  # sums over ranks; pass 2 divides the means by world and uses the GLOBAL (sum m / numel)^2
+            dist.all_reduce(red)  # sums over ranks; pass 2 divides the means by world and uses the GLOBAL (sum m / numel)^2
 
         # ---- pass 2 (loss assembly + history matching on the device, remaining loss gradients) and the backward ------
         total = ops.empty(N)
         pub = ops.empty(len(self._dirs), N, 8)
+        if be_on:
+            be_pub = ops.empty(nd, N)
+            be_weights = [float(w) for w in be_w] + [0.0] * (N - len(be_w))  # 0: this member's gate is closed
         matching = bool(self.do_w_loss_matching)
         for di, d in enumerate(self._dirs):
             rec = fw[d]
@@ -599,6 +631,9 @@ class Council_Trainer(nn.Module):
                 ops.acc_slice(d_x, d_x8, 4)
             if d_x is None:
                 d_x = ops.zeros(*rec['x_fake'].shape)
+            if be_on:  # after gen_loss_bwd of this direction: the totals share its accumulator
+                ops.abs_beginning_end_bwd(rec['x_fake'], self._src(d, img_a, img_b), be_sums[di], hpd['numel'], be_weights, total,
+                                          be_pub[di], d_x)
             gen.backward(d_x, d_mask, rec['enc'], rec['dec'],
                          on_decoder_done=(lambda g=gen: self._reduce_async('gen', g, g.enc_end, None))
                          if self.world > 1 and os.environ.get('COUNCIL_DP_SYNC') != '1' else None)
@@ -629,6 +664,9 @@ class Council_Trainer(nn.Module):
                 setattr(self, 'loss_gen_mask_total_%s_s' % ab, [])
                 setattr(self, 'loss_gen_mask_TV_%s_s' % ab, [])
                 setattr(self, 'council_loss_%s_s' % ab, [])
+        if be_w is not None:  # :477-484: one entry per member whose gate was open, the int 0 for an inactive direction
+            for d, name in (('a2b', 'loss_gen_beginning_end_a_ab_s'), ('b2a', 'loss_gen_beginning_end_b_ba_s')):
+                setattr(self, name, [be_pub[self._dirs.index(d), i] for i in range(len(be_w))] if d in fw else [0] * len(be_w))
         self._last_fw = {d: {'x_fake': fw[d]['x_fake'], 'mask': fw[d]['mask']} for d in self._dirs}
 
     # ==================================================================================================

@@ -174,7 +174,8 @@ int cg_focus_fwd(const float* mask, float* sums, int G, int B, int H, int W, flo
 int cg_focus_bwd(const float* mask, const float* coef, float* dmask, int G, int B, int H, int W,
                  float center, float eps, void* stream);
 
-/* ---- fused losses (one launch per discriminator update and direction; two per gen_update and direction) ----------
+/* ---- fused losses (one launch per discriminator update and direction; two per gen_update and direction, two more with
+ *      abs_beginning_end on) --------------------------------------------------------------------------------------------
  * These replace the four calls above on the training path: the loss of EVERY discriminator scale, the focus terms, the
  * loss-history matching and all their gradients, with no host round trip (trainer_council.py:518-524,576-586 run on the
  * device).  `ws`: >= cg_loss_workspace_bytes() bytes, ZERO-INITIALISED once by the caller, not shared between streams;
@@ -224,6 +225,20 @@ int cg_gen_loss_fwd(const cg_gen_loss_desc* d, float* scal, void* ws, size_t ws_
 int cg_gen_loss_bwd(const cg_gen_loss_desc* d, const cg_gen_loss_hp* hp, const float* scal, double* hist_gan,
                     double* hist_council, float* total, int accumulate, float* pub, float* d_mask, void* ws,
                     size_t ws_bytes, void* stream);
+/* abs_beginning_end: recon_criterion_v2_color(x_fake, x) (trainer_council.py:210-215, 477-495) with d = x_fake - x over the 3 live
+ * lanes of x_fake[G][B][H][W][4] and the shared x[1][B][H][W][4] (the generator's input); loss = L1 = mean |d| if L1 > L2 = mean d^2,
+ * else L2 (a tie picks L2).
+ * pass 1: sums[G][2] = { sum |d|, sum d^2 } for this rank (float partials per block, added in double; fixed order). */
+int cg_abs_beginning_end_fwd(const float* x_fake, const float* x, float* sums, int G, int B, int H, int W, void* ws,
+                             size_t ws_bytes, void* stream);
+/* pass 2 (sums summed over ranks; numel = 3*H*W*B of the GLOBAL minibatch): the branch is chosen from the sums on the device;
+ * pub[g] = unweighted loss; d_x (+)= host_weight[g] * (sign(d) / numel  or  2d / numel) on lanes 0..2 (sign(0) = 0);
+ * total[g] (+)= host_weight[g] * loss through the double accumulator cg_gen_loss_bwd keeps in the same workspace, so it must
+ * follow the cg_gen_loss_bwd call of the same direction on the same workspace and stream.  host_weight[G] (host memory) is
+ * passed to the kernel by value; 0 leaves total and d_x of that member untouched. */
+int cg_abs_beginning_end_bwd(const float* x_fake, const float* x, const float* sums, double numel, const double* host_weight,
+                             float* total, float* pub, float* d_x, int G, int B, int H, int W, void* ws, size_t ws_bytes,
+                             void* stream);
 size_t cg_loss_workspace_bytes(int G, int B, int H, int W);
 
 /* plumbing: p[0:bytes] = 0 on `stream` (cudaMemsetAsync; keeps framework fill kernels out of the launch list) */
