@@ -408,6 +408,95 @@ __global__ void __launch_bounds__(256) abs_be_bwd_kernel(const float* __restrict
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// gen_update, latent reconstruction (recon_c_w / recon_s_w, trainer_council.py:359-369, 460-469): recon_criterion = mean |a - b|
+// of a re-encoded content / style code a against its target b
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int L1_THREADS = 256, L1_MAX_BLOCKS = 256;  // blocks per member
+
+// block (j, g) walks member g's n elements with stride nb * 256 (fixed for a shape: the float partial of a block and therefore the
+// sum are deterministic); the last block adds each member's partials in double, in block order.  The gradient does not depend on
+// the loss value: da (+)= coef * sign(a - b), db (+)= -coef * sign(a - b) in the same pass (sign(0) = 0).
+template <bool VEC>
+__global__ void __launch_bounds__(L1_THREADS) latent_l1_kernel(const float* __restrict__ a, const float* __restrict__ b, int b_shared, long n,
+                                                               float* __restrict__ da, float* __restrict__ db, float coef, int accumulate,
+                                                               float* __restrict__ sums, float* __restrict__ part,
+                                                               unsigned int* __restrict__ counter, int G, int nb) {
+    pdl_trigger();
+    pdl_wait();
+    __shared__ float sm[32];
+    const int g = blockIdx.x / nb, j = blockIdx.x - g * nb;
+    const long base = (long)g * n, bbase = b_shared ? 0 : base;
+    float v[1] = {0.f};
+    if (VEC) {
+        const long n4 = n / 4;
+        const float4* a4 = reinterpret_cast<const float4*>(a + base);
+        const float4* b4 = reinterpret_cast<const float4*>(b + bbase);
+        float4* da4 = da ? reinterpret_cast<float4*>(da + base) : nullptr;
+        float4* db4 = db ? reinterpret_cast<float4*>(db + base) : nullptr;
+        for (long i = (long)j * L1_THREADS + threadIdx.x; i < n4; i += (long)nb * L1_THREADS) {
+            const float4 x = __ldg(a4 + i), y = __ldg(b4 + i);
+            const float d0 = x.x - y.x, d1 = x.y - y.y, d2 = x.z - y.z, d3 = x.w - y.w;
+            v[0] += fabsf(d0) + fabsf(d1) + fabsf(d2) + fabsf(d3);
+            const float4 gr = make_float4(coef * sgnf(d0), coef * sgnf(d1), coef * sgnf(d2), coef * sgnf(d3));
+            if (da4) {
+                float4 o = accumulate ? da4[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+                o.x += gr.x; o.y += gr.y; o.z += gr.z; o.w += gr.w;
+                da4[i] = o;
+            }
+            if (db4) {
+                float4 o = accumulate ? db4[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+                o.x -= gr.x; o.y -= gr.y; o.z -= gr.z; o.w -= gr.w;
+                db4[i] = o;
+            }
+        }
+    } else {
+        for (long i = (long)j * L1_THREADS + threadIdx.x; i < n; i += (long)nb * L1_THREADS) {
+            const float d = __ldg(a + base + i) - __ldg(b + bbase + i);
+            v[0] += fabsf(d);
+            const float gr = coef * sgnf(d);
+            if (da) da[base + i] = (accumulate ? da[base + i] : 0.f) + gr;
+            if (db) db[base + i] = (accumulate ? db[base + i] : 0.f) - gr;
+        }
+    }
+    block_sum<1>(v, sm);
+    if (threadIdx.x == 0) part[blockIdx.x] = v[0];
+    if (!last_block_done(counter, gridDim.x)) return;
+    if (threadIdx.x < G) {
+        const volatile float* vp = part + (long)threadIdx.x * nb;
+        double s = 0.0;
+        for (int k = 0; k < nb; k++) s += (double)vp[k];
+        sums[threadIdx.x] = (float)s;
+    }
+    if (threadIdx.x == 0) *counter = 0u;
+}
+
+struct ReconTerms { double numel[CG_RECON_MAX_TERMS], w[CG_RECON_MAX_TERMS]; };
+
+// after the all-reduce: pub[k][g] = sums[k][g] / numel[k]; total[g] += sum_k w[k] * pub[k][g] through the double accumulator of
+// the direction totals (the one cg_gen_loss_bwd keeps in the same workspace)
+__global__ void recon_finalize_kernel(const float* __restrict__ sums, const ReconTerms t, int nterm, int G, float* __restrict__ total,
+                                      double* __restrict__ total64, float* __restrict__ pub) {
+    pdl_trigger();
+    pdl_wait();
+    const int g = threadIdx.x;
+    if (g >= G) return;
+    double t64 = total64[g];
+    bool any = false;
+    for (int k = 0; k < nterm; k++) {
+        const double val = (double)sums[k * G + g] / t.numel[k];
+        pub[k * G + g] = (float)val;
+        if (t.w[k] != 0.0) {
+            t64 += t.w[k] * val;
+            any = true;
+        }
+    }
+    if (any) {
+        total64[g] = t64;
+        total[g] = (float)t64;
+    }
+}
+
 }  // namespace cg
 
 using namespace cg;
@@ -524,4 +613,44 @@ extern "C" int cg_abs_beginning_end_bwd(const float* x_fake, const float* x, con
     if (blocks > cap) blocks = cap;
     launch_k(abs_be_bwd_kernel, blocks, 256, 0, ST, x_fake, x, sums, numel, wt, G, npix, total, ws_total64(ws), pub, d_x);
     return check_launch("abs_beginning_end_bwd");
+}
+
+static int latent_l1_blocks(long n) {
+    const long units = n % 4 == 0 ? n / 4 : n;
+    int nb = cdiv(units, (long)L1_THREADS * 8);
+    return nb < 1 ? 1 : (nb > L1_MAX_BLOCKS ? L1_MAX_BLOCKS : nb);
+}
+
+extern "C" int cg_latent_l1(const float* a, const float* b, int b_shared, float* da, float* db, float coef, int accumulate, float* sums,
+                            int G, long n, void* ws, size_t ws_bytes, void* stream) {
+    CG_REQUIRE(a && b && sums && G >= 1 && G <= CG_LOSS_MAX_G && n >= 1, "latent_l1: G=%d n=%ld out of range", G, n);
+    CG_REQUIRE(!(db && b_shared), "latent_l1: a target shared by all members cannot take a gradient");
+    const int nb = latent_l1_blocks(n);
+    size_t need = 16 + CG_LOSS_MAX_G * 8 + (size_t)G * nb * 4;
+    if (need > ws_bytes) {
+        set_error("latent_l1: workspace %zu < %zu bytes", ws_bytes, need);
+        return CG_ERR_WORKSPACE;
+    }
+    if (n % 4 == 0)
+        launch_k(latent_l1_kernel<true>, G * nb, L1_THREADS, 0, ST, a, b, b_shared, n, da, db, coef, accumulate, sums, ws_part(ws),
+                 ws_counter(ws), G, nb);
+    else
+        launch_k(latent_l1_kernel<false>, G * nb, L1_THREADS, 0, ST, a, b, b_shared, n, da, db, coef, accumulate, sums, ws_part(ws),
+                 ws_counter(ws), G, nb);
+    return check_launch("latent_l1");
+}
+
+extern "C" int cg_recon_finalize(const float* sums, const double* host_numel, const double* host_weight, int nterm, int G, float* total,
+                                 float* pub, void* ws, size_t ws_bytes, void* stream) {
+    CG_REQUIRE(sums && host_numel && host_weight && total && pub && nterm >= 1 && nterm <= CG_RECON_MAX_TERMS && G >= 1 &&
+               G <= CG_LOSS_MAX_G, "recon_finalize: nterm=%d G=%d out of range", nterm, G);
+    CG_REQUIRE(ws_bytes >= 16 + CG_LOSS_MAX_G * 8, "recon_finalize: workspace too small");
+    ReconTerms t = {};
+    for (int k = 0; k < nterm; k++) {
+        CG_REQUIRE(host_numel[k] > 0, "recon_finalize: numel must be positive");
+        t.numel[k] = host_numel[k];
+        t.w[k] = host_weight[k];
+    }
+    launch_k(recon_finalize_kernel, 1, 32, 0, ST, sums, t, nterm, G, total, ws_total64(ws), pub);
+    return check_launch("recon_finalize");
 }

@@ -169,6 +169,39 @@ __global__ void avgpool_bwd_kernel(const float* __restrict__ dy, float* __restri
     for (int c = 0; c < nch; c++) o[c] = accumulate ? o[c] + acc[c] : acc[c];
 }
 
+// style encoder tail (networks.py:348: nn.AdaptiveAvgPool2d(1)): one thread per (image, channel) sums its HW pixels in pixel order
+__global__ void global_avgpool_fwd_kernel(const float* __restrict__ h, float* __restrict__ y, int N, int HW, int C) {
+    pdl_trigger();
+    pdl_wait();
+    long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (long)N * C) return;
+    const long n = i / C;
+    const int c = (int)(i - n * C);
+    const float* p = h + n * HW * (long)C + c;
+    float s = 0.f;
+    for (int k = 0; k < HW; k++) s += __ldg(p + (long)k * C);
+    y[i] = s / (float)HW;
+}
+
+// dh = dy / HW at every pixel, times the ReLU gate h > 0 when relu_gate (h: the pool's input, a ReLU output)
+__global__ void global_avgpool_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ h, float* __restrict__ dh, long total4,
+                                          int HW, int C4, int relu_gate) {
+    pdl_trigger();
+    pdl_wait();
+    long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total4) return;
+    const long n = i / ((long)HW * C4);
+    const int c = (int)(i % C4);
+    const float r = 1.f / (float)HW;
+    float4 g = __ldg(reinterpret_cast<const float4*>(dy) + n * C4 + c);
+    g.x *= r; g.y *= r; g.z *= r; g.w *= r;
+    if (relu_gate) {
+        const float4 v = __ldg(reinterpret_cast<const float4*>(h) + i);
+        g.x = v.x > 0.f ? g.x : 0.f; g.y = v.y > 0.f ? g.y : 0.f; g.z = v.z > 0.f ? g.z : 0.f; g.w = v.w > 0.f ? g.w : 0.f;
+    }
+    reinterpret_cast<float4*>(dh)[i] = g;
+}
+
 __global__ void acc_slice_kernel(float* __restrict__ dst, const float* __restrict__ src, long npix, int Cd, int Cs, int nch) {
     pdl_trigger();
     pdl_wait();
@@ -373,6 +406,18 @@ extern "C" int cg_avgpool_bwd(const float* dy, float* dx, int N, int H, int W, i
     long total = (long)N * H * W;
     launch_k(avgpool_bwd_kernel, cdiv(total, 256), 256, 0, ST, dy, dx, total, H, W, Cy, Cx, nch, accumulate);
     return check_launch("avgpool_bwd");
+}
+extern "C" int cg_global_avgpool_fwd(const float* h, float* y, int N, int HW, int C, void* stream) {
+    CG_REQUIRE(h && y && N >= 1 && HW >= 1 && C >= 1, "global_avgpool_fwd: N=%d HW=%d C=%d out of range", N, HW, C);
+    launch_k(global_avgpool_fwd_kernel, cdiv((long)N * C, 256), 256, 0, ST, h, y, N, HW, C);
+    return check_launch("global_avgpool_fwd");
+}
+extern "C" int cg_global_avgpool_bwd(const float* dy, const float* h, float* dh, int N, int HW, int C, int relu_gate, void* stream) {
+    CG_REQUIRE(dy && dh && (h || !relu_gate) && N >= 1 && HW >= 1 && C >= 4 && C % 4 == 0,
+               "global_avgpool_bwd: N=%d HW=%d C=%d out of range (C must be a multiple of 4)", N, HW, C);
+    const long total4 = (long)N * HW * (C / 4);
+    launch_k(global_avgpool_bwd_kernel, cdiv(total4, 256), 256, 0, ST, dy, h, dh, total4, HW, C / 4, relu_gate);
+    return check_launch("global_avgpool_bwd");
 }
 extern "C" int cg_acc_slice(float* dst, const float* src, long npix, int Cd, int Cs, int nch, void* stream) {
     launch_k(acc_slice_kernel, cdiv(npix, 256), 256, 0, ST, dst, src, npix, Cd, Cs, nch);

@@ -288,7 +288,8 @@ class CouncilGen(_StackedNet):
         self.mlp = [LayerSpec('mlp.model.0.fc', self.mlp_dim, self.style_dim, 1, 1, 0, linear=True),
                     LayerSpec('mlp.model.1.fc', self.mlp_dim, self.mlp_dim, 1, 1, 0, linear=True),
                     LayerSpec('mlp.model.2.fc', self.n_adain, self.mlp_dim, 1, 1, 0, linear=True)]
-        # --- style encoder (networks.py:337-350): parameters kept for the API / checkpoints, never stepped
+        # --- style encoder (networks.py:337-350): run by encode() / sample(), and in training only by the style reconstruction
+        # (recon_s_w != 0), the one term that gives it a gradient; otherwise its parameters are kept for the API / checkpoints
         d = dim
         self.sty = [LayerSpec('enc_style.model.0.conv', d, input_dim, 7, 1, 3, lanes=img_lanes)]
         for i in range(2):
@@ -305,16 +306,32 @@ class CouncilGen(_StackedNet):
         # flat-buffer offset where the content encoder's parameters end: the decoder / head / MLP gradients [enc_end:] are
         # complete before the encoder backward starts, so data parallelism all-reduces them while it runs
         self.enc_end = self.bank.table[self.dec_res[0][0].wname][0] if self.dec_res else self.bank.table[self.head[0].wname][0]
-        self.frozen = ParamBank(ops, G, [e for s in self.sty + [self.sty_out] for e in s.entries()], trainable=False)
+        # its own bank: gradients, Adam moments and step count only when recon_s_w trains it (torch's Adam starts a parameter's
+        # state at its first gradient, so this bank's step count can lag the generator's, e.g. after resuming with the term off)
+        self.sty_bank = ParamBank(ops, G, [e for s in self.sty + [self.sty_out] for e in s.entries()],
+                                  trainable=hp.get('recon_s_w', 0) != 0)
         # biases feeding IN / AdaIN are mathematically dead (SURVEY.md 7.3-5): their gradient is exactly 0 here
         self.dead_bias = set(s.bname for s in live if s not in self.head and s not in self.mlp)
+        self._enc_grad2 = None
+
+    @property
+    def frozen(self):  # the style-encoder bank's earlier name
+        return self.sty_bank
+
+    def reencode_grad(self):
+        """Zero-initialised flat buffer laid out like bank.grad[:enc_end]: the content encoder's weight gradients of its second pass
+        in gen_update (the re-encode of the other direction's translation), added to bank.grad after the first pass's backward.
+        The dead biases are never written, so they stay 0."""
+        if self._enc_grad2 is None:
+            self._enc_grad2 = self.ops.zeros(self.enc_end)
+        return self._enc_grad2
 
     # -- state_dict plumbing -------------------------------------------------------------------------
     def _specs(self):
         return self.sty + [self.sty_out] + self.live_specs
 
     def _banks(self):
-        return (self.bank, self.frozen)
+        return (self.bank, self.sty_bank)
 
     def extra_state(self):
         out = OrderedDict()
@@ -375,15 +392,15 @@ class CouncilGen(_StackedNet):
             saved.append((x, y, mean, rstd))
         return z
 
-    def _conv_norm_bwd(self, dz, s, rec, adain, d_adain, act, ups_out, addend, need_dx=True):
-        """Backward of _conv_norm: fills the weight gradient, returns d(input).  With ups_out, dz has the
-        upsampled shape and the 2x2 fan-in is summed while it is read."""
+    def _conv_norm_bwd(self, dz, s, rec, adain, d_adain, act, ups_out, addend, need_dx=True, grad=None):
+        """Backward of _conv_norm: fills the weight gradient (in bank.grad, or in the flat buffer grad laid out like it), returns
+        d(input).  With ups_out, dz has the upsampled shape and the 2x2 fan-in is summed while it is read."""
         ops = self.ops
         x, y, mean, rstd = rec
         off = self.adain_off.get(s.key, 0)
         norm_bwd = ops.norm_fused_bwd if self.coop_norm_bwd else ops.norm_act_bwd
         dy = norm_bwd(dz, y, mean, rstd, adain, off, act, ups_out, d_adain)
-        ops.conv_wgrad(x, dy, self.bank.g(s.wname), None, s.stride, s.pad)
+        ops.conv_wgrad(x, dy, self.bank.g(s.wname) if grad is None else self.bank._view(grad, s.wname), None, s.stride, s.pad)
         if not need_dx:
             return None
         return ops.conv_dgrad(dy, self.bank.p(s.wname), x.shape, s.stride, s.pad, addend=addend)
@@ -449,9 +466,10 @@ class CouncilGen(_StackedNet):
         return x_fake, mask
 
     # -- backward (gen_update only) -------------------------------------------------------------------
-    def backward(self, d_xfake, d_mask, enc_saved, dec_saved, on_decoder_done=None):
+    def backward(self, d_xfake, d_mask, enc_saved, dec_saved, on_decoder_done=None, d_content=None):
         """Fills ``self.bank.grad`` for every live parameter given d(loss)/d(x_fake), d(loss)/d(mask).
-        on_decoder_done: called when grad[enc_end:] (decoder, head, MLP) is final, before the encoder backward."""
+        on_decoder_done: called when grad[enc_end:] (decoder, head, MLP) is final, before the encoder backward.
+        d_content: a further gradient of the content code (the recon_c target), added to what the decoder sends back."""
         ops, bank = self.ops, self.bank
         dec_saved = list(dec_saved)
         adain, acts, x_img = dec_saved.pop()
@@ -491,18 +509,26 @@ class CouncilGen(_StackedNet):
                 dm = ops.conv_dgrad(dm, bank.p(s.wname), h_in.shape, 1, 0, mask_src=h_in, mask_slope=0.0)
         if on_decoder_done is not None:
             on_decoder_done()
-        # content encoder
+        if d_content is not None:
+            ops.add_(d, d_content)
+        self.encode_backward(d, enc_saved)
+
+    def encode_backward(self, d, enc_saved, grad=None, want_dx=False, addend=None):
+        """Backward of encode(x, enc_saved) from d(content): weight gradients into bank.grad (or the flat buffer grad laid out like
+        it); returns d(x) + addend when want_dx (x: a per-member image [G,B,H,W,4]), else None."""
         recs = list(enc_saved)
         k = len(recs) - 1
         for blk in reversed(self.enc_res):
             d_out = d
-            d = self._conv_norm_bwd(d_out, blk[1], recs[k], None, None, ACT_NONE, False, None)
-            d = self._conv_norm_bwd(d, blk[0], recs[k - 1], None, None, ACT_RELU, False, d_out)
+            d = self._conv_norm_bwd(d_out, blk[1], recs[k], None, None, ACT_NONE, False, None, grad=grad)
+            d = self._conv_norm_bwd(d, blk[0], recs[k - 1], None, None, ACT_RELU, False, d_out, grad=grad)
             k -= 2
         for li in range(len(self.enc) - 1, -1, -1):
-            d = self._conv_norm_bwd(d, self.enc[li], recs[k], None, None, ACT_RELU, False, None, need_dx=li > 0)
+            d = self._conv_norm_bwd(d, self.enc[li], recs[k], None, None, ACT_RELU, False, addend if li == 0 else None,
+                                    need_dx=li > 0 or want_dx, grad=grad)
             k -= 1
         assert k == -1
+        return d
 
     # -- single-member API (reference's gen.encode / gen.decode on NCHW tensors) -----------------------
     def member_encode(self, i, images):
@@ -513,20 +539,45 @@ class CouncilGen(_StackedNet):
         content = ops.nhwc_to_nchw(c[0], self.cdim)
         return content, self.member_style_encode(i, x)
 
-    def style_encode(self, x, sl=None):
+    def style_encode(self, x, sl=None, saved=None):
         """StyleEncoder networks.py:337-353 (norm none, relu), all members (or member sl) at once:
-        x [1,B,H,W,4] -> style codes [G,B,1,1,style_dim].  Not on the training path (its result is discarded there)."""
-        ops, fz = self.ops, self.frozen
+        x [1|G,B,H,W,4] -> style codes [G,B,1,1,style_dim].  In training only the style reconstruction (recon_s_w) runs it, on the
+        other direction's translations; saved (a list) keeps what style_backward needs."""
+        ops, sb = self.ops, self.sty_bank
 
         def wb(s):
-            w, b = fz.p(s.wname), fz.p(s.bname)
+            w, b = sb.p(s.wname), sb.p(s.bname)
             return (w, b) if sl is None else (w[sl:sl + 1], b[sl:sl + 1])
+        acts = [x]
         h = x
         for s in self.sty:
             h = ops.conv_fwd(h, *wb(s), s.stride, s.pad, act=ACT_RELU)
-        # global average pool (tiny, plumbing) then the 1x1 conv as a linear layer
-        pooled = h.mean(dim=(2, 3), keepdim=True).contiguous()
+            acts.append(h)
+        # global average pool, then the 1x1 conv as a linear layer.  Training (saved) pools with the library's kernel, which
+        # style_backward differentiates; the no-grad API path (encode(), sample()) keeps the tensor mean it has always used, so its
+        # results are unchanged and op sets without the pool op can still serve it.
+        if saved is not None:
+            pooled = ops.global_avgpool_fwd(h)
+            saved.extend([acts, pooled])
+        else:
+            pooled = h.mean(dim=(2, 3), keepdim=True).contiguous()
         return ops.conv_fwd(pooled, *wb(self.sty_out), 1, 0)
+
+    def style_backward(self, d_s, saved, addend=None):
+        """Backward of style_encode(x, saved=saved) from d(style code) [G,B,1,1,S]: weight and bias gradients into sty_bank.grad;
+        returns d(x) [G,B,H,W,4] (+ addend)."""
+        ops, sb = self.ops, self.sty_bank
+        acts, pooled = saved
+        s = self.sty_out
+        ops.conv_wgrad(pooled, d_s, sb.g(s.wname), sb.g(s.bname), 1, 0)
+        d = ops.conv_dgrad(d_s, sb.p(s.wname), pooled.shape, 1, 0)
+        d = ops.global_avgpool_bwd(d, acts[-1])  # gated by the last layer's ReLU
+        for li in range(len(self.sty) - 1, -1, -1):
+            s = self.sty[li]
+            ops.conv_wgrad(acts[li], d, sb.g(s.wname), sb.g(s.bname), s.stride, s.pad)
+            d = ops.conv_dgrad(d, sb.p(s.wname), acts[li].shape, s.stride, s.pad, addend=addend if li == 0 else None,
+                               mask_src=acts[li] if li > 0 else None, mask_slope=0.0)
+        return d
 
     def member_style_encode(self, i, x):
         """-> [B, style_dim, 1, 1] of member i (AdaINGen.encode's second result, networks.py:278-283)."""

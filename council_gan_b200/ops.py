@@ -87,6 +87,11 @@ _SIGS = {
     'cg_abs_beginning_end_fwd': (C.c_int, [_fp, _fp, _fp] + [C.c_int] * 4 + [_fp, C.c_size_t, _fp]),
     'cg_abs_beginning_end_bwd': (C.c_int, [_fp, _fp, _fp, C.c_double, C.POINTER(C.c_double), _fp, _fp, _fp] + [C.c_int] * 4 +
                                  [_fp, C.c_size_t, _fp]),
+    'cg_latent_l1': (C.c_int, [_fp, _fp, C.c_int, _fp, _fp, C.c_float, C.c_int, _fp, C.c_int, C.c_long, _fp, C.c_size_t, _fp]),
+    'cg_recon_finalize': (C.c_int, [_fp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int, C.c_int, _fp, _fp, _fp, C.c_size_t,
+                                    _fp]),
+    'cg_global_avgpool_fwd': (C.c_int, [_fp, _fp, C.c_int, C.c_int, C.c_int, _fp]),
+    'cg_global_avgpool_bwd': (C.c_int, [_fp, _fp, _fp, C.c_int, C.c_int, C.c_int, C.c_int, _fp]),
     'cg_loss_workspace_bytes': (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int]),
     'cg_zero': (C.c_int, [_fp, C.c_size_t, _fp]),
     'cg_aug_color': (C.c_int, [_fp, _fp, _fp, _fp, _fp, C.c_int, C.c_int, C.c_int, _fp]),
@@ -450,6 +455,31 @@ class CudaOps:
         self._ck(self.lib.cg_avgpool_bwd(_p(dy), _p(dx), G * B, H, W, dy.shape[-1], Cx, nch, int(bool(accumulate)),
                                          self._stream()), 'cg_avgpool_bwd')
 
+    def global_avgpool_fwd(self, h):
+        """h [G,B,H,W,C] -> [G,B,1,1,C], the mean over H x W (the style encoder's nn.AdaptiveAvgPool2d(1))"""
+        self._chk(h)
+        G, B, H, W, Cc = h.shape
+        y = self.empty(G, B, 1, 1, Cc)
+        self._ck(self.lib.cg_global_avgpool_fwd(_p(h), _p(y), G * B, H * W, Cc, self._stream()), 'cg_global_avgpool_fwd')
+        return y
+
+    def global_avgpool_bwd(self, dy, h, relu_gate=True):
+        """dy [G,B,1,1,C], h [G,B,H,W,C] (the pooled ReLU output) -> dh = dy / HW, gated by h > 0 when relu_gate"""
+        self._chk(dy, h)
+        G, B, H, W, Cc = h.shape
+        assert tuple(dy.shape) == (G, B, 1, 1, Cc)
+        dh = self.empty(G, B, H, W, Cc)
+        self._timed_raw('hbm:global_avgpool_bwd G%d B%d %dx%d C%d' % (G, B, H, W, Cc), 4.0 * (2 if relu_gate else 1) * h.numel(),
+                        lambda: self._ck(self.lib.cg_global_avgpool_bwd(_p(dy), _p(h), _p(dh), G * B, H * W, Cc, int(bool(relu_gate)),
+                                                                        self._stream()), 'cg_global_avgpool_bwd'))
+        return dh
+
+    def add_(self, dst, src):
+        """dst += src elementwise (contiguous tensors of the same size), one launch"""
+        self._chk(dst, src)
+        assert dst.numel() == src.numel()
+        self._ck(self.lib.cg_acc_slice(_p(dst), _p(src), dst.numel(), 1, 1, 1, self._stream()), 'cg_acc_slice')
+
     def acc_slice(self, dst, src, nch):
         self._chk(dst, src)
         npix = dst.numel() // dst.shape[-1]
@@ -653,6 +683,32 @@ class CudaOps:
         ws = self._loss_scratch(G)  # never grows the scratch: a new buffer would drop the accumulator gen_loss_bwd left in it
         self._ck(self.lib.cg_abs_beginning_end_bwd(_p(x_fake), _p(x), _p(sums), float(numel), w, _p(total), _p(pub), _p(d_x), G, B, H, W,
                                                    _p(ws), ws.numel(), self._stream()), 'cg_abs_beginning_end_bwd')
+
+    def latent_l1(self, a, b, sums, coef, da=None, db=None, accumulate=False):
+        """recon_criterion(a, b) = mean |a - b| per member (recon_c / recon_s): sums[g] = sum |a - b| of member g on this rank; in the
+        same launch da (+)= coef * sign(a - b) and db (+)= -coef * sign(a - b) (None: not wanted).  a [G, ...]; b [G, ...] of the same
+        shape, or [1, ...] shared by all members (then db must be None)."""
+        self._chk(a, b, sums, da, db)
+        G = a.shape[0]
+        n = a.numel() // G
+        shared = b.shape[0] == 1 and G > 1
+        assert b.numel() == (n if shared else a.numel()) and sums.numel() == G
+        for t in (da, db):
+            assert t is None or t.numel() == a.numel()
+        ws = self._loss_scratch(G)
+        self._timed_raw('hbm:latent_l1 G%d n%d' % (G, n), 4.0 * a.numel() * (2 + (da is not None) + (db is not None)),
+                        lambda: self._ck(self.lib.cg_latent_l1(_p(a), _p(b), int(shared), _p(da), _p(db), float(coef), int(bool(accumulate)),
+                                                               _p(sums), G, n, _p(ws), ws.numel(), self._stream()), 'cg_latent_l1'))
+
+    def recon_finalize(self, sums, numel, weights, total, pub):
+        """After the all-reduce: pub[k, g] = sums[k, g] / numel[k]; total[g] += sum_k weights[k] * pub[k, g] through gen_loss_bwd's
+        double accumulator (so it follows every gen_loss_bwd call of the update).  sums, pub [K, G]; numel, weights: K python floats."""
+        self._chk(sums, total, pub)
+        K, G = sums.shape
+        assert len(numel) == len(weights) == K and tuple(pub.shape) == (K, G)
+        ws = self._loss_scratch(G)  # never grows the scratch: a new buffer would drop the accumulator gen_loss_bwd left in it
+        self._ck(self.lib.cg_recon_finalize(_p(sums), (C.c_double * K)(*numel), (C.c_double * K)(*weights), K, G, _p(total), _p(pub),
+                                            _p(ws), ws.numel(), self._stream()), 'cg_recon_finalize')
 
     # -- input pipeline (council_gan_b200/data.py) ------------------------------------------------------
     def aug_color(self, pix, desc, opcode, param, B, max_pixels, any_contrast):

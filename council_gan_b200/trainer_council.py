@@ -28,8 +28,16 @@ What is different underneath (GPU-first, see DESIGN.md):
     weight are host arithmetic on Python floats (``abs_beginning_end_w_conf``, with the reference's member-0 quirk); its value,
     branch (L1 or L2) and gradient are two more launches per direction (csrc/losses.cu) whose sums join the scalar all-reduce.
     With ``abs_beginning_end: 0`` (the shipped configs) nothing of it runs.
-Paths outside the live configuration space of the reference's three configs (recon_*/vgg/council_abs losses,
-nsgan/RaHinge, do_my_style, gray-scale D, random D/G pairing) raise NotImplementedError.
+  * recon_c_w / recon_s_w (:359-369, 460-469, the latent reconstructions; both directions required): after both forwards each
+    translation is re-encoded by the other direction's generator (content encoder for recon_c, style encoder for recon_s).
+    One launch per term computes mean |recon - target| and its gradient; the sums join the scalar all-reduce and one launch
+    after pass 2 publishes ``loss_gen_recon_{s,c}_{a,b}_s`` and adds the weighted values to the totals.  The re-encode
+    backward runs before either generator's own backward: its d(x_fake) joins d_x, the recon_c target gradient joins the
+    content gradient, and the content encoder's weight gradients of its two passes are summed.  recon_s_w is the only term
+    that trains the style encoder; its bank then has its own Adam state.  With both weights 0 (the shipped configs) nothing
+    of it runs.
+Paths outside the live configuration space of the reference's three configs (recon_x / recon_x_cyc / vgg / council_abs
+losses, nsgan/RaHinge, do_my_style, gray-scale D, random D/G pairing) raise NotImplementedError.
 """
 from __future__ import annotations
 
@@ -220,9 +228,12 @@ class Council_Trainer(nn.Module):
     # ------------------------------------------------------------------------------------------------
     @staticmethod
     def _check_supported(hp):
-        bad = [k for k in ('recon_x_w', 'recon_s_w', 'recon_c_w', 'recon_x_cyc_w', 'vgg_w', 'council_abs_w') if hp.get(k, 0) != 0]
+        bad = [k for k in ('recon_x_w', 'recon_x_cyc_w', 'vgg_w', 'council_abs_w') if hp.get(k, 0) != 0]
         if bad:
             raise NotImplementedError('loss terms %s are not on the accelerated training path' % bad)
+        if (hp.get('recon_c_w', 0) != 0 or hp.get('recon_s_w', 0) != 0) and not (hp['do_a2b'] and hp['do_b2a']):
+            raise NotImplementedError('recon_c_w / recon_s_w re-encode each translation with the other direction\'s generator, so '
+                                      'they need do_a2b and do_b2a (with one direction the reference fails with an IndexError)')
         if hp['dis']['gan_type'] != 'lsgan':
             assert 0, "Unsupported GAN type: {}".format(hp['dis']['gan_type'])
         if hp['dis'].get('do_Dis_only_gray') or hp['dis'].get('useRandomGen') or hp['gen'].get('useRandomDis'):
@@ -340,14 +351,16 @@ class Council_Trainer(nn.Module):
         return self._lr0 * self._gamma ** (self._sched_epoch[fam] // self._step_size)
 
     # ---- optimiser step, data-parallel gradient exchange ---------------------------------------------------
-    def _reduce_async(self, fam, net, lo=0, hi=None):
-        """Queue the all-reduce of grad[lo:hi] of one network (NCCL stream, ordered after everything issued so far)."""
+    def _reduce_async(self, fam, net, lo=0, hi=None, bank=None):
+        """Queue the all-reduce of grad[lo:hi] of one bank of a network (default: its main bank; NCCL stream, ordered after
+        everything issued so far)."""
         dist = _dist()
         work = None
+        bank = net.bank if bank is None else bank
         if dist is not None and self.world > 1:
-            g = net.bank.grad if (lo == 0 and hi is None) else net.bank.grad[lo:hi]
+            g = bank.grad if (lo == 0 and hi is None) else bank.grad[lo:hi]
             work = dist.all_reduce(g, async_op=True)  # SUM; local coefficients already carry 1/world
-        self._pending.setdefault(fam, []).append((net, work))
+        self._pending.setdefault(fam, []).append((net, bank, work))
 
     def _finish(self, fam):
         """Join the family's queued all-reduces (stream-side wait, no host block on NCCL) and run its fused Adam."""
@@ -356,15 +369,14 @@ class Council_Trainer(nn.Module):
             return
         if hasattr(self.ops, 'wgrad_join'):
             self.ops.wgrad_join()  # weight gradients may have been queued on a side stream (COUNCIL_WGRAD_STREAM=1)
-        for _, work in items:
+        for _, _, work in items:
             if work is not None:
                 work.wait()  # every bucket of the family first
         done = []
-        for net, _ in items:
-            if any(net is n for n in done):
-                continue  # a network with several buckets steps once
-            done.append(net)
-            bank = net.bank
+        for net, bank, _ in items:
+            if any(bank is b for b in done):
+                continue  # a bank with several buckets steps once
+            done.append(bank)
             bank.step += 1
             self.ops.adam_step(bank.data, bank.grad, bank.exp_avg, bank.exp_avg_sq, self._lr(fam), self._betas[0],
                                self._betas[1], 1e-8, self._wd, bank.step)
@@ -386,7 +398,7 @@ class Council_Trainer(nn.Module):
             net = self._nets.get('%s_%s' % (fam, d))
             if net is None:
                 continue
-            if not any(net is n for n, _ in self._pending.get(fam, [])):
+            if not any(net.bank is b for _, b, _ in self._pending.get(fam, [])):
                 self._reduce_async(fam, net)
         if not (defer and self.world > 1) or os.environ.get('COUNCIL_DP_SYNC') == '1':  # COUNCIL_DP_SYNC=1: A/B switch, join immediately
             self._finish(fam)
@@ -557,13 +569,24 @@ class Council_Trainer(nn.Module):
         center, eps = float(fl['mask_zero_or_one_center']), float(fl['mask_zero_or_one_epsilon'])
         be_w = self._abs_beginning_end_weights(hp, iterations)
         be_on = bool(be_w)
+        # latent reconstruction (:359-369, 460-469): the terms in the reference's list order, as (kind, domain, weight); the
+        # translation of direction d is re-encoded by the other direction's generator
+        recon = ([('s', 'a', hp['recon_s_w']), ('s', 'b', hp['recon_s_w'])] if hp['recon_s_w'] != 0 else []) + \
+                ([('c', 'a', hp['recon_c_w']), ('c', 'b', hp['recon_c_w'])] if hp['recon_c_w'] != 0 else [])
+        if hp['recon_s_w'] != 0 and not all(self._nets['gen_' + d].sty_bank.trainable for d in self._dirs):
+            raise NotImplementedError('recon_s_w trains the style encoder: it must be non-zero when the trainer is built')
 
         # ---- forward of every direction; pass 1 of the loss (all reductions, one launch per direction) -----------
         fw = {}
         nd = len(self._dirs)
-        if be_on:  # the abs_beginning_end sums [|d|, d^2] ride behind the other scalars: still one all-reduce
-            red = ops.empty(nd * N * 8)
-            scal, be_sums = red[:nd * N * 6].view(nd, N, 6), red[nd * N * 6:].view(nd, N, 2)
+        extra = (nd * N * 2 if be_on else 0) + len(recon) * N
+        if extra:  # the abs_beginning_end sums [|d|, d^2] and the recon sums ride behind the other scalars: still one all-reduce
+            red = ops.empty(nd * N * 6 + extra)
+            scal, off = red[:nd * N * 6].view(nd, N, 6), nd * N * 6
+            if be_on:
+                be_sums, off = red[off:off + nd * N * 2].view(nd, N, 2), off + nd * N * 2
+            if recon:
+                rc_sums = red[off:].view(len(recon), N)
         else:
             red = scal = ops.empty(nd, N, 6)  # per direction and member: [adv, council, focus sums x4] of THIS rank
         for di, d in enumerate(self._dirs):
@@ -591,11 +614,16 @@ class Council_Trainer(nn.Module):
                                             float(hp['gan_w']) / self.world, scal[di])
             if be_on:
                 ops.abs_beginning_end_fwd(x_fake, src, be_sums[di])
+            if recon:
+                rec['c'] = c
             fw[d] = rec
+        if recon:
+            recon_numel = self._recon_forward(fw, s, recon, rc_sums)
         self._flush()  # (a family gated off above still steps here)
         dist = _dist()
         if dist is not None and self.world > 1:
             dist.all_reduce(red)  # sums over ranks; pass 2 divides the means by world and uses the GLOBAL (sum m / numel)^2
+        d_x_re = self._recon_backward(fw, recon) if recon else {}
 
         # ---- pass 2 (loss assembly + history matching on the device, remaining loss gradients) and the backward ------
         total = ops.empty(N)
@@ -629,6 +657,11 @@ class Council_Trainer(nn.Module):
                 if d_x is None:
                     d_x = ops.zeros(*rec['x_fake'].shape)
                 ops.acc_slice(d_x, d_x8, 4)
+            if d in d_x_re:  # d(recon) / d(x_fake) through the other generator's re-encode
+                if d_x is None:
+                    d_x = d_x_re[d]
+                else:
+                    ops.add_(d_x, d_x_re[d])
             if d_x is None:
                 d_x = ops.zeros(*rec['x_fake'].shape)
             if be_on:  # after gen_loss_bwd of this direction: the totals share its accumulator
@@ -636,9 +669,14 @@ class Council_Trainer(nn.Module):
                                           be_pub[di], d_x)
             gen.backward(d_x, d_mask, rec['enc'], rec['dec'],
                          on_decoder_done=(lambda g=gen: self._reduce_async('gen', g, g.enc_end, None))
-                         if self.world > 1 and os.environ.get('COUNCIL_DP_SYNC') != '1' else None)
+                         if self.world > 1 and os.environ.get('COUNCIL_DP_SYNC') != '1' else None, d_content=rec.get('d_c'))
+            if 'd_c' in rec:  # the content encoder ran twice: add the re-encode pass's weight gradients
+                ops.add_(gen.bank.grad[:gen.enc_end], gen.reencode_grad())
             if self.world > 1 and os.environ.get('COUNCIL_DP_SYNC') != '1':
                 self._reduce_async('gen', gen, 0, gen.enc_end)  # encoder bucket; the decoder bucket went out during the encoder backward
+        if recon:  # after every gen_loss_bwd / abs_beginning_end_bwd of this update: the member totals share their accumulator
+            rc_pub = ops.empty(len(recon), N)
+            ops.recon_finalize(rc_sums, recon_numel, [float(w) for _, _, w in recon], total, rc_pub)
         self._adam('gen', defer=True)  # joined at the start of the next update (or by save / state_dict / sample)
         self._enc_cache.clear()
 
@@ -667,7 +705,59 @@ class Council_Trainer(nn.Module):
         if be_w is not None:  # :477-484: one entry per member whose gate was open, the int 0 for an inactive direction
             for d, name in (('a2b', 'loss_gen_beginning_end_a_ab_s'), ('b2a', 'loss_gen_beginning_end_b_ba_s')):
                 setattr(self, name, [be_pub[self._dirs.index(d), i] for i in range(len(be_w))] if d in fw else [0] * len(be_w))
+        if recon:  # :310-313, :460-469: one entry per member, [] for a term whose weight is 0
+            for kind in ('s', 'c'):
+                for dom in ('a', 'b'):
+                    setattr(self, 'loss_gen_recon_%s_%s_s' % (kind, dom), [])
+            for k, (kind, dom, _) in enumerate(recon):
+                setattr(self, 'loss_gen_recon_%s_%s_s' % (kind, dom), [rc_pub[k, i] for i in range(N)])
         self._last_fw = {d: {'x_fake': fw[d]['x_fake'], 'mask': fw[d]['mask']} for d in self._dirs}
+
+    def _recon_forward(self, fw, s, recon, sums):
+        """Re-encode each translation with the other direction's generator (:359-369), keeping activations for the backward, and
+        evaluate the latent reconstruction terms: sums[k] = this rank's sum |recon - target| of term k, written together with the
+        gradients (they do not depend on the loss value).  -> numel of each term over the GLOBAL minibatch."""
+        ops = self.ops
+        other = {'a2b': 'b2a', 'b2a': 'a2b'}
+        numel = []
+        for k, (kind, dom, w) in enumerate(recon):
+            # recon_c_a / recon_s_b come from re-encoding x_ab (direction a2b), recon_c_b / recon_s_a from x_ba
+            d = ('a2b' if dom == 'a' else 'b2a') if kind == 'c' else ('a2b' if dom == 'b' else 'b2a')
+            rec = fw[d]
+            gen_o = self._nets['gen_' + other[d]]
+            if kind == 'c':  # mean |c_recon - c|; the target c is not detached (:466-467): it takes the opposite gradient
+                rec['c_saved'] = []
+                c_rec = gen_o.encode(rec['x_fake'], rec['c_saved'])
+                n = rec['c'][0].numel() * self.world
+                rec['d_c_rec'], rec['d_c'] = ops.empty(*c_rec.shape), ops.empty(*c_rec.shape)
+                ops.latent_l1(c_rec, rec['c'], sums[k], float(w) / n, da=rec['d_c_rec'], db=rec['d_c'])
+            else:  # mean |s_recon - s|, s the style noise this direction decoded with
+                rec['s_saved'] = []
+                s_rec = gen_o.style_encode(rec['x_fake'], saved=rec['s_saved'])
+                n = s[d][0].numel() * self.world
+                rec['d_s_rec'] = ops.empty(*s_rec.shape)
+                ops.latent_l1(s_rec, s[d], sums[k], float(w) / n, da=rec['d_s_rec'])
+            numel.append(float(n))
+        return numel
+
+    def _recon_backward(self, fw, recon):
+        """Backward of both re-encodes, before either generator's own backward: the other generator's style-encoder gradients (then
+        queued for its all-reduce) and content-encoder gradients (into its reencode_grad() buffer), and d(recon) / d(x_fake) of every
+        direction that has a term."""
+        other = {'a2b': 'b2a', 'b2a': 'a2b'}
+        d_x = {}
+        for d in self._dirs:
+            rec = fw[d]
+            gen_o = self._nets['gen_' + other[d]]
+            dx = None
+            if 's_saved' in rec:
+                dx = gen_o.style_backward(rec['d_s_rec'], rec['s_saved'])
+                self._reduce_async('gen', gen_o, bank=gen_o.sty_bank)
+            if 'c_saved' in rec:
+                dx = gen_o.encode_backward(rec['d_c_rec'], rec['c_saved'], grad=gen_o.reencode_grad(), want_dx=True, addend=dx)
+            if dx is not None:
+                d_x[d] = dx
+        return d_x
 
     # ==================================================================================================
     # the rest of the reference surface
@@ -774,7 +864,7 @@ class Council_Trainer(nn.Module):
     def _load_opt_state_dict(self, fam, i, sd):
         """Inverse of _opt_state_dict; accepts what torch.optim.Adam.state_dict() of the reference wrote (:988-992)."""
         plist = self._opt_params(fam)
-        steps = []
+        steps = {}  # bank -> largest step of its entries
         for idx, ent in sd.get('state', {}).items():
             net, spec, is_w = plist[int(idx)]
             name = spec.wname if is_w else spec.bname
@@ -787,14 +877,22 @@ class Council_Trainer(nn.Module):
                     spec.import_weight(dst, ent[key])
                 else:
                     dst.copy_(ent[key].detach().to('cpu', dst.dtype).reshape(-1))
-            steps.append(int(float(ent['step'])))
-        return max(steps) if steps else None
+            steps[bank] = max(steps.get(bank, 0), int(float(ent['step'])))
+        return steps
 
     def resume(self, checkpoint_dir, hyperparameters):
         """Load the latest per-member checkpoints (:898-967); returns the iteration parsed from the file name."""
         self._flush()
         iterations = 0
-        steps = {}  # the flat Adam keeps ONE step count per family (the reference: one per parameter, all equal in practice)
+        # the flat Adam keeps ONE step count per family for the main banks (the reference: one per parameter, all equal in practice)
+        # and one per style-encoder bank, whose parameters have state only once recon_s_w has given them a gradient
+        steps = {}
+        sty_steps = {}
+        for d in self._dirs:
+            sb = self._nets['gen_' + d].sty_bank
+            if sb.trainable:  # a checkpoint without style-encoder entries (written with the term off) starts its moments at zero
+                sb.exp_avg, sb.exp_avg_sq, sb.step = self.ops.zeros(sb.total), self.ops.zeros(sb.total), 0
+                sty_steps[sb] = 0
         for i in range(self.council_size):
             for fam in ('gen', 'dis', 'dis_council'):
                 if fam == 'dis_council' and not self.do_dis_council:
@@ -815,15 +913,19 @@ class Council_Trainer(nn.Module):
             try:
                 opt = torch.load(opt_path, map_location='cpu')
                 for fam in ('dis', 'gen') + (('dis_council',) if self.do_dis_council else ()):
-                    st = self._load_opt_state_dict(fam, i, opt[fam])
-                    if st is not None:
-                        steps[fam] = max(steps.get(fam, 0), st)
+                    for bank, st in self._load_opt_state_dict(fam, i, opt[fam]).items():
+                        if bank in sty_steps:
+                            sty_steps[bank] = max(sty_steps[bank], st)
+                        else:
+                            steps[fam] = max(steps.get(fam, 0), st)
             except Exception as e:  # the reference warns and carries on as well (:958-959)
                 import warnings
                 warnings.warn('some optimizer FAILED to load (%s: %s): Adam moments restart from zero' % (type(e).__name__, e))
         for fam, st in steps.items():
             for d in self._dirs:
                 self._nets['%s_%s' % (fam, d)].bank.step = st
+        for bank, st in sty_steps.items():
+            bank.step = st
         if iterations > 0:
             print('Resume from iteration %d' % iterations)
             for fam in self._sched_epoch:  # get_scheduler(..., last_epoch=iterations) :953-957

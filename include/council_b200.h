@@ -143,6 +143,10 @@ int cg_head_fused(const float* y, const float* mean, const float* rstd, const fl
 /* ---- image-space helpers ---------------------------------------------------------------------- */
 /* nn.AvgPool2d(3, 2, padding=1, count_include_pad=False), networks.py:32,129 */
 int cg_avgpool_fwd(const float* x, float* y, int N, int H, int W, int C, void* stream);
+/* global average pool of the style encoder (networks.py:348): y[N][C] = mean over HW of h[N][HW][C] (pixel-order float sum / HW);
+ * backward: dh[N][HW][C] = dy[N][C] / HW, zeroed where h <= 0 when relu_gate (h: the ReLU output that was pooled); C % 4 == 0 */
+int cg_global_avgpool_fwd(const float* h, float* y, int N, int HW, int C, void* stream);
+int cg_global_avgpool_bwd(const float* dy, const float* h, float* dh, int N, int HW, int C, int relu_gate, void* stream);
 /* dx[N][H][W][Cx] (first nch lanes) = or += avgpool^T(dy[N][H/2][W/2][Cy] first nch lanes) */
 int cg_avgpool_bwd(const float* dy, float* dx, int N, int H, int W, int Cy, int Cx, int nch,
                    int accumulate, void* stream);
@@ -239,6 +243,19 @@ int cg_abs_beginning_end_fwd(const float* x_fake, const float* x, float* sums, i
 int cg_abs_beginning_end_bwd(const float* x_fake, const float* x, const float* sums, double numel, const double* host_weight,
                              float* total, float* pub, float* d_x, int G, int B, int H, int W, void* ws, size_t ws_bytes,
                              void* stream);
+/* latent reconstruction, recon_c_w / recon_s_w (trainer_council.py:359-369, 460-469): recon_criterion(a, b) = mean |a - b| of a
+ * re-encoded code a[G][n] against its target b ([G][n], or [n] shared by all members when b_shared).
+ * sums[g] = sum |a - b| over member g on this rank (float partials per block, added in double; fixed order), and in the same pass
+ * da (+)= coef * sign(a - b), db (+)= -coef * sign(a - b) (sign(0) = 0; NULL: not wanted; accumulate 0 writes, 1 adds) with
+ * coef = w / numel of the GLOBAL minibatch.  db needs a per-member b. */
+int cg_latent_l1(const float* a, const float* b, int b_shared, float* da, float* db, float coef, int accumulate, float* sums,
+                 int G, long n, void* ws, size_t ws_bytes, void* stream);
+#define CG_RECON_MAX_TERMS 4
+/* after the all-reduce of sums[nterm][G]: pub[k][g] = sums[k][g] / host_numel[k]; total[g] += sum_k host_weight[k] * pub[k][g]
+ * through the double accumulator cg_gen_loss_bwd keeps in the same workspace (so it must follow the cg_gen_loss_bwd calls of
+ * this update on that workspace and stream).  host_numel / host_weight (host memory) are passed by value. */
+int cg_recon_finalize(const float* sums, const double* host_numel, const double* host_weight, int nterm, int G, float* total,
+                      float* pub, void* ws, size_t ws_bytes, void* stream);
 size_t cg_loss_workspace_bytes(int G, int B, int H, int W);
 
 /* plumbing: p[0:bytes] = 0 on `stream` (cudaMemsetAsync; keeps framework fill kernels out of the launch list) */
