@@ -132,7 +132,7 @@ extern "C" int cg_set_tensor_core_mode(int mode) {
     g_tc_mode = mode == 1 ? 7 : (mode & 7);  // 1 = everything; otherwise a bit mask: 1 forward, 2 data gradient, 4 weight gradient
     g_small_bn = ((mode >> 23) & 1) ? 0 : 1;  // bit 23: keep the widest N tile even when the launch has fewer tiles than SMs
     g_wgrad_tma = ((mode >> 25) & 1) ? 0 : 1;  // bit 25: stride-1 weight gradients on wgrad_tc_kernel instead of wgrad_tma_kernel
-    g_pdl = ((mode >> 22) & 1) ? 1 : (((mode >> 24) & 1) ? 2 : 0);  // bit 22: programmatic dependent launch; bit 24: for the helper kernels only
+    g_pdl = (mode >> 22) & 1;  // bit 22: programmatic dependent launch
     return prev;
 }
 

@@ -58,7 +58,7 @@ static inline int cdiv(long a, long b) { return (int)((a + b - 1) / b); }
 // exactly those of plain stream order (every kernel waits, so completion is transitive along the stream).  Kernels of other libraries
 // (NCCL, memsets, copies) are launched without the attribute and keep full stream serialisation on both sides.
 // Early-scheduled dependents cost more than the launch gaps they hide once kernels are long, so the attribute is OFF unless mode
-// bit 22 asks for it (the trainer does on small, launch-bound maps: COUNCIL_PDL=auto|0|1).
+// bit 22 asks for it (the trainer does on small, launch-bound maps).
 extern thread_local int g_pdl;
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -72,8 +72,7 @@ inline void launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem,
     cfg.stream = st;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    // g_pdl: 0 off, 1 every kernel, 2 only the helper kernels (no dynamic shared memory: transforms, finalisers, reductions, pointwise passes)
-    at[0].val.programmaticStreamSerializationAllowed = (g_pdl == 1 || (g_pdl == 2 && smem == 0)) ? 1 : 0;
+    at[0].val.programmaticStreamSerializationAllowed = g_pdl;
     cfg.attrs = at;
     cfg.numAttrs = 1;
     (void)cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);  // errors surface through check_launch()'s cudaGetLastError

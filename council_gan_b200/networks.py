@@ -18,7 +18,6 @@ Per-member ``state_dict`` views keep the reference's key names and OIHW shapes (
 from __future__ import annotations
 
 import math
-import os
 from collections import OrderedDict
 
 import torch
@@ -237,15 +236,6 @@ class CouncilGen(_StackedNet):
         assert g['pad_type'] == 'zero' and g['activ'] == 'relu'
         assert input_dim == 3 and g['num_of_mask_dim_to_add'] == 3, 'mask head kernel is specialised for RGB + 3 masks'
         self.ops, self.hp, self.G = ops, hp, G
-        # statistics in the convolution epilogue (cg_conv_fwd_stats) vs a separate pass.
-        # '1': every normalised layer; 'auto' (default): the wide layers (>= 128 output channels, K >= 1024), whose main loop is an order of
-        # magnitude longer than the epilogue and hides the reduction; '0': never (the narrow full-resolution layers are epilogue-bound).
-        self.fuse_stats = os.environ.get('COUNCIL_FUSE_STATS', 'auto')
-        # single-launch normalisation with L2-resident second pass (csrc/norm_coop.cu): correct and tested, opt-in: COUNCIL_COOP_NORM=1
-        coop = os.environ.get('COUNCIL_COOP_NORM', '0')  # 0 | 1 (forward and backward) | bwd (backward only: keeps the statistics epilogue)
-        self.coop_norm = coop == '1'
-        self.coop_norm_bwd = coop in ('1', 'bwd')
-        self.fuse_head = os.environ.get('COUNCIL_FUSE_HEAD', '1') == '1'  # decoder tail of no-grad passes as one kernel (csrc/head_fused.cu)
         self.dim, self.style_dim, self.nd, self.nr, self.mlp_dim = g['dim'], g['style_dim'], g['n_downsample'], g['n_res'], g['mlp_dim']
         dim, nd, nr = self.dim, self.nd, self.nr
         img_lanes = [0, 1, 2]
@@ -377,17 +367,16 @@ class CouncilGen(_StackedNet):
         # the bias of a convolution that feeds IN / AdaIN is removed again by the mean subtraction: skip the add
         # ups_in (no-grad passes): the x2 nearest upsample is folded into this convolution (four 2x2 parity classes)
         off = self.adain_off.get(s.key, 0)
+        # statistics in the convolution epilogue (cg_conv_fwd_stats) on the wide layers (>= 128 output channels, K >= 1024), whose main
+        # loop is an order of magnitude longer than the epilogue and hides the reduction; a separate pass on the narrow
+        # full-resolution layers, which are epilogue-bound
         wide = s.cout >= 128 and s.k * s.k * s.cin >= 1024
-        if self.fuse_stats == '1' or (self.fuse_stats == 'auto' and wide and not self.coop_norm):
+        if wide:
             y, mean, rstd = ops.conv_fwd_stats(x, w, s.stride, s.pad, ups=ups_in)
-            z = ops.norm_act_fwd(y, mean, rstd, adain, off, res, act, ups_out)
-        elif self.coop_norm:  # statistics + normalise in one launch, second pass over y from L2 (csrc/norm_coop.cu)
-            y = ops.conv_fwd(x, w, None, s.stride, s.pad, ups=ups_in)
-            z, mean, rstd = ops.norm_fused_fwd(y, adain, off, res, act, ups_out)
         else:
             y = ops.conv_fwd(x, w, None, s.stride, s.pad, ups=ups_in)
             mean, rstd = ops.in_stats(y)
-            z = ops.norm_act_fwd(y, mean, rstd, adain, off, res, act, ups_out)
+        z = ops.norm_act_fwd(y, mean, rstd, adain, off, res, act, ups_out)
         if saved is not None:
             saved.append((x, y, mean, rstd))
         return z
@@ -398,8 +387,7 @@ class CouncilGen(_StackedNet):
         ops = self.ops
         x, y, mean, rstd = rec
         off = self.adain_off.get(s.key, 0)
-        norm_bwd = ops.norm_fused_bwd if self.coop_norm_bwd else ops.norm_act_bwd
-        dy = norm_bwd(dz, y, mean, rstd, adain, off, act, ups_out, d_adain)
+        dy = ops.norm_act_bwd(dz, y, mean, rstd, adain, off, act, ups_out, d_adain)
         ops.conv_wgrad(x, dy, self.bank.g(s.wname) if grad is None else self.bank._view(grad, s.wname), None, s.stride, s.pad)
         if not need_dx:
             return None
@@ -446,7 +434,7 @@ class CouncilGen(_StackedNet):
             x = self._conv_norm(x, blk[1], sl, adain, ACT_NONE, res, r == nres - 1 and nup > 0 and not fold, saved)
         for u, (a, b) in enumerate(self.dec_up):
             x = self._conv_norm(x, a, sl, adain, ACT_RELU, None, False, saved, ups_in=fold)
-            if fold and u + 1 == nup and self.fuse_head and b.cout == 64 and ops.head_fused_supported((1, 1, x.shape[2], x.shape[3], 64)):
+            if fold and u + 1 == nup and b.cout == 64 and ops.head_fused_supported((1, 1, x.shape[2], x.shape[3], 64)):
                 # no-grad pass: the rest of the decoder (AdaIN + ReLU of this block, the three 1x1 head layers, mask compositing)
                 # is one kernel; the 64-channel full-resolution map is read once instead of making four HBM round trips
                 w, _ = self._w(b, sl)

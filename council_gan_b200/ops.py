@@ -64,9 +64,6 @@ _SIGS = {
     'cg_in_stats': (C.c_int, [_fp, _fp, _fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, _fp, C.c_size_t, _fp]),
     'cg_norm_act_fwd': (C.c_int, [_fp, _fp, _fp, _fp, C.c_int, C.c_int, _fp, _fp] + [C.c_int] * 7 + [_fp]),
     'cg_norm_act_bwd': (C.c_int, [_fp, _fp, _fp, _fp, _fp, C.c_int, C.c_int, _fp, _fp] + [C.c_int] * 7 + [_fp, C.c_size_t, _fp]),
-    'cg_norm_fused_fwd': (C.c_int, [_fp, _fp, C.c_int, C.c_int, _fp, _fp, _fp, _fp] + [C.c_int] * 7 + [C.c_float, _fp, C.c_size_t, _fp]),
-    'cg_norm_fused_bwd': (C.c_int, [_fp, _fp, _fp, _fp, _fp, C.c_int, C.c_int, _fp, _fp] + [C.c_int] * 7 + [_fp, C.c_size_t, _fp]),
-    'cg_norm_fused_workspace_bytes': (C.c_size_t, [C.c_int] * 3),
     'cg_upsample2x_bwd': (C.c_int, [_fp, _fp, C.c_int, C.c_int, C.c_int, C.c_int, _fp]),
     'cg_mask_head_fwd': (C.c_int, [_fp, _fp, _fp, _fp, C.c_int, C.c_int, C.c_int, _fp]),
     'cg_head_fused': (C.c_int, [_fp, _fp, _fp, _fp, C.c_int, C.c_int] + [_fp] * 9 + [C.c_int] * 3 + [_fp]),
@@ -150,11 +147,6 @@ class CudaOps:
         self._stage_ring = [None] * 8
         self._ws_sizes = {}
         self._stage_next = 0
-        # experimental (round 2, not yet measured): weight gradients on a side stream so that they overlap the HBM-bound passes of
-        # the main stream.  bank.grad is written only by conv_wgrad and read only after wgrad_join() (trainer _adam).
-        self._wgrad_stream = torch.cuda.Stream(self.device) if os.environ.get('COUNCIL_WGRAD_STREAM', '0') == '1' else None
-        self._ws_side = None
-        self._stream_cached = None
 
     # -- plumbing ---------------------------------------------------------------------------------
     def _stream(self):
@@ -309,27 +301,9 @@ class CudaOps:
         self._chk(x, dy, dw, db)
         g = self._geom(x.shape, dw, stride, pad, ups)
         assert tuple(dy.shape) == (g.G, g.B, g.Ho, g.Wo, g.Cout)
-        side = self._wgrad_stream
-        if side is None:
-            ws = self._conv_ws(g, 2)
-            self._timed('conv_wgrad', g, lambda: self._ck(self.lib.cg_conv_wgrad(
-                C.byref(g), _p(x), _p(dy), _p(dw), _p(db), _p(ws), ws.numel(), self._stream()), 'cg_conv_wgrad'))
-            return
-        need = self.lib.cg_conv_workspace_bytes(C.byref(g), 2)
-        side.wait_stream(torch.cuda.current_stream(self.device))  # x and dy were produced on the main stream
-        with torch.cuda.stream(side):
-            if self._ws_side is None or need > self._ws_side.numel():
-                self._ws_side = torch.empty(max(int(need * 1.25) + 1024, 64 << 20), dtype=torch.uint8, device=self.device)
-            ws = self._ws_side
-            self._timed('conv_wgrad', g, lambda: self._ck(self.lib.cg_conv_wgrad(
-                C.byref(g), _p(x), _p(dy), _p(dw), _p(db), _p(ws), ws.numel(), side.cuda_stream), 'cg_conv_wgrad'))
-        for t in (x, dy):
-            t.record_stream(side)  # the caching allocator must not hand their memory out before the side stream is done
-
-    def wgrad_join(self):
-        """Order everything queued on the weight-gradient side stream before what the main stream does next."""
-        if self._wgrad_stream is not None:
-            torch.cuda.current_stream(self.device).wait_stream(self._wgrad_stream)
+        ws = self._conv_ws(g, 2)
+        self._timed('conv_wgrad', g, lambda: self._ck(self.lib.cg_conv_wgrad(
+            C.byref(g), _p(x), _p(dy), _p(dw), _p(db), _p(ws), ws.numel(), self._stream()), 'cg_conv_wgrad'))
 
     # -- instance norm / AdaIN --------------------------------------------------------------------
     def in_stats(self, y, eps=1e-5):
@@ -365,37 +339,6 @@ class CudaOps:
                         lambda: self._ck(self.lib.cg_norm_act_bwd(_p(dz), _p(y), _p(mean), _p(rstd), _p(adain), P, off, _p(dy), _p(d_adain),
                                                                   G, B, H, W, Cc, act, int(bool(ups)), _p(ws), ws.numel(), self._stream()),
                                          'cg_norm_act_bwd'))
-        return dy
-
-    # single-launch forms (csrc/norm_coop.cu): HBM sees y once, the second pass is served from L2
-    def norm_fused_fwd(self, y, adain=None, off=0, res=None, act=ACT_NONE, ups=False, eps=1e-5):
-        """statistics + normalise (+AdaIN affine, +activation, +residual, +x2 upsample) in ONE launch -> (z, mean, rstd)"""
-        self._chk(y, adain, res)
-        G, B, H, W, Cc = y.shape
-        z = self.empty(G, B, 2 * H if ups else H, 2 * W if ups else W, Cc)
-        mean, rstd = self.empty(G, B, Cc), self.empty(G, B, Cc)
-        P = adain.shape[-1] if adain is not None else 0
-        ws = self._ws_for(self.lib.cg_norm_fused_workspace_bytes(G, B, Cc))
-        units = 1 + (1 if res is not None else 0) + (4 if ups else 1)  # HBM: read y once (+ residual), write z (x4 when upsampling)
-        self._timed_raw('hbm:norm_fused_fwd G%d B%d %dx%d C%d%s%s' % (G, B, H, W, Cc, ' res' if res is not None else '', ' ups' if ups else ''),
-                        4.0 * units * y.numel(),
-                        lambda: self._ck(self.lib.cg_norm_fused_fwd(_p(y), _p(adain), P, off, _p(res), _p(z), _p(mean), _p(rstd), G, B, H, W, Cc,
-                                                                    act, int(bool(ups)), eps, _p(ws), ws.numel(), self._stream()),
-                                         'cg_norm_fused_fwd'))
-        return z, mean, rstd
-
-    def norm_fused_bwd(self, dz, y, mean, rstd, adain=None, off=0, act=ACT_NONE, ups=False, d_adain=None):
-        """both reductions + apply of the normalisation backward in ONE launch -> dy (d_adain columns overwritten)"""
-        self._chk(dz, y, mean, rstd, adain, d_adain)
-        G, B, H, W, Cc = y.shape
-        dy = self.empty(G, B, H, W, Cc)
-        P = adain.shape[-1] if adain is not None else 0
-        ws = self._ws_for(self.lib.cg_norm_fused_workspace_bytes(G, B, Cc))
-        units = 1 + (4 if ups else 1) + 1  # HBM: read y and dz once, write dy
-        self._timed_raw('hbm:norm_fused_bwd G%d B%d %dx%d C%d%s' % (G, B, H, W, Cc, ' ups' if ups else ''), 4.0 * units * y.numel(),
-                        lambda: self._ck(self.lib.cg_norm_fused_bwd(_p(dz), _p(y), _p(mean), _p(rstd), _p(adain), P, off, _p(dy), _p(d_adain),
-                                                                    G, B, H, W, Cc, act, int(bool(ups)), _p(ws), ws.numel(), self._stream()),
-                                         'cg_norm_fused_bwd'))
         return dy
 
     def upsample2x_bwd(self, d_up):

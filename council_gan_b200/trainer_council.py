@@ -64,7 +64,6 @@ def _dist():
     return None
 
 
-_PDL = os.environ.get('COUNCIL_PDL', 'auto')   # auto | 0 | 1
 _PDL_MAX_PIXELS = 128 * 128 * 4             # batch x height x width up to which programmatic dependent launch is switched on
 
 
@@ -76,14 +75,13 @@ def _pinned(fn):
         if not hasattr(ops, 'pin_stream') or ops._stream_cached is not None:
             return fn(self, *args, **kwargs)
         ops.pin_stream()
-        if _PDL != 'auto':
-            ops.set_pdl(_PDL == '1')
-        else:  # launch-bound small maps only: early-scheduled dependents cost more than the launch gaps they hide once kernels are long
-            for x in args:
-                if torch.is_tensor(x):
-                    pix = x.numel() // (IMG_C if x.dim() == 5 else max(int(x.shape[1]), 1)) if x.dim() >= 4 else 0
-                    ops.set_pdl(0 < pix <= _PDL_MAX_PIXELS)
-                    break
+        # programmatic dependent launch on launch-bound small maps only: early-scheduled dependents cost more than the launch gaps
+        # they hide once kernels are long
+        for x in args:
+            if torch.is_tensor(x):
+                pix = x.numel() // (IMG_C if x.dim() == 5 else max(int(x.shape[1]), 1)) if x.dim() >= 4 else 0
+                ops.set_pdl(0 < pix <= _PDL_MAX_PIXELS)
+                break
         try:
             return fn(self, *args, **kwargs)
         finally:
@@ -367,8 +365,6 @@ class Council_Trainer(nn.Module):
         items = self._pending.pop(fam, None)
         if not items:
             return
-        if hasattr(self.ops, 'wgrad_join'):
-            self.ops.wgrad_join()  # weight gradients may have been queued on a side stream (COUNCIL_WGRAD_STREAM=1)
         for _, _, work in items:
             if work is not None:
                 work.wait()  # every bucket of the family first
@@ -400,7 +396,7 @@ class Council_Trainer(nn.Module):
                 continue
             if not any(net.bank is b for _, b, _ in self._pending.get(fam, [])):
                 self._reduce_async(fam, net)
-        if not (defer and self.world > 1) or os.environ.get('COUNCIL_DP_SYNC') == '1':  # COUNCIL_DP_SYNC=1: A/B switch, join immediately
+        if not (defer and self.world > 1):
             self._finish(fam)
 
     def _src(self, d, a, b):
@@ -632,6 +628,7 @@ class Council_Trainer(nn.Module):
             be_pub = ops.empty(nd, N)
             be_weights = [float(w) for w in be_w] + [0.0] * (N - len(be_w))  # 0: this member's gate is closed
         matching = bool(self.do_w_loss_matching)
+        data_parallel = self.world > 1
         for di, d in enumerate(self._dirs):
             rec = fw[d]
             gen = self._nets['gen_' + d]
@@ -669,10 +666,10 @@ class Council_Trainer(nn.Module):
                                           be_pub[di], d_x)
             gen.backward(d_x, d_mask, rec['enc'], rec['dec'],
                          on_decoder_done=(lambda g=gen: self._reduce_async('gen', g, g.enc_end, None))
-                         if self.world > 1 and os.environ.get('COUNCIL_DP_SYNC') != '1' else None, d_content=rec.get('d_c'))
+                         if data_parallel else None, d_content=rec.get('d_c'))
             if 'd_c' in rec:  # the content encoder ran twice: add the re-encode pass's weight gradients
                 ops.add_(gen.bank.grad[:gen.enc_end], gen.reencode_grad())
-            if self.world > 1 and os.environ.get('COUNCIL_DP_SYNC') != '1':
+            if data_parallel:
                 self._reduce_async('gen', gen, 0, gen.enc_end)  # encoder bucket; the decoder bucket went out during the encoder backward
         if recon:  # after every gen_loss_bwd / abs_beginning_end_bwd of this update: the member totals share their accumulator
             rc_pub = ops.empty(len(recon), N)

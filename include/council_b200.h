@@ -57,8 +57,8 @@ int cg_device_info(int* sm_count, int* cc_major, int* cc_minor);
 /* 0 = SIMT fp32 kernels only; 1 (default) = TF32 tensor-core kernels (wgmma / mma.sync) wherever a layer qualifies;
  * other values are a bit mask for bring-up: 2 = data gradient only, 4 = weight gradient only, ...
  * (internally 1 forward | 2 dgrad | 4 wgrad).  Switches on top of the mask: 1<<22 = programmatic dependent launch between this
- * library's kernels (every kernel carries the griddepcontrol pair; the trainer turns it on for small maps only), 1<<24 = programmatic
- * dependent launch for the helper kernels only (those without dynamic shared memory), 1<<23 = keep the widest N tile on small maps
+ * library's kernels (every kernel carries the griddepcontrol pair; the trainer turns it on for small maps only),
+ * 1<<23 = keep the widest N tile on small maps
  * (default: narrower tiles when a launch has fewer tiles than SMs), 1<<25 = weight gradients of stride-1 and stride-2 KxK layers
  * on the previous tensor-core kernel, which transposes both operands in the MMA warps, for comparisons in one process (default:
  * the TMA-fed kernel that reads one operand from a channel-major copy).  Other bits are accepted and ignored.
@@ -108,18 +108,6 @@ int cg_norm_act_fwd(const float* y, const float* mean, const float* rstd, const 
 int cg_norm_act_bwd(const float* dz, const float* y, const float* mean, const float* rstd,
                     const float* adain, int P, int off, float* dy, float* d_adain, int G, int B,
                     int H, int W, int C, int act, int ups, void* ws, size_t ws_bytes, void* stream);
-
-/* Single-launch forms of the three calls above (csrc/norm_coop.cu): statistics + normalise in ONE kernel, and the whole
- * backward in ONE kernel; a launch keeps only as many instances in flight as fit in L2, so the second pass over y (and dz)
- * is served from L2 and HBM sees y once.  Same results as cg_in_stats + cg_norm_act_fwd / cg_norm_act_bwd; mean / rstd
- * [G][B][C] are also written by the forward (the backward needs them).  ws >= cg_norm_fused_workspace_bytes(). */
-int cg_norm_fused_fwd(const float* y, const float* adain, int P, int off, const float* res, float* z, float* mean,
-                      float* rstd, int G, int B, int H, int W, int C, int act, int ups, float eps, void* ws,
-                      size_t ws_bytes, void* stream);
-int cg_norm_fused_bwd(const float* dz, const float* y, const float* mean, const float* rstd, const float* adain, int P,
-                      int off, float* dy, float* d_adain, int G, int B, int H, int W, int C, int act, int ups, void* ws,
-                      size_t ws_bytes, void* stream);
-size_t cg_norm_fused_workspace_bytes(int G, int B, int C);
 
 /* backward of nn.Upsample(scale_factor=2) (networks.py:385): dx[N][H][W][C] = 2x2 fan-in sum of d_up[N][2H][2W][C] */
 int cg_upsample2x_bwd(const float* d_up, float* dx, int N, int H, int W, int C, void* stream);

@@ -134,13 +134,6 @@ class TorchOps:
             dy, = torch.autograd.grad(z, [yy], dz)
         return dy.contiguous()
 
-    def norm_fused_fwd(self, y, adain=None, off=0, res=None, act=ACT_NONE, ups=False, eps=1e-5):
-        mean, rstd = self.in_stats(y, eps)
-        return self.norm_act_fwd(y, mean, rstd, adain, off, res, act, ups), mean, rstd
-
-    def norm_fused_bwd(self, dz, y, mean, rstd, adain=None, off=0, act=ACT_NONE, ups=False, d_adain=None):
-        return self.norm_act_bwd(dz, y, mean, rstd, adain, off, act, ups, d_adain)
-
     def upsample2x_bwd(self, d_up):
         G, B, H2, W2, Cc = d_up.shape
         return d_up.reshape(G, B, H2 // 2, 2, W2 // 2, 2, Cc).sum(dim=(3, 5)).contiguous()

@@ -203,7 +203,7 @@ def test_weight_init_statistics():
 
 def test_update_pins_the_stream_and_picks_pdl_by_batch_size():
     """host logic of the launch path: an update resolves the stream once (ops.pin_stream / unpin_stream around the call, also when it
-    raises) and turns programmatic dependent launch on only for small batches (COUNCIL_PDL=auto)."""
+    raises) and turns programmatic dependent launch on only for small batches."""
     from council_gan_b200 import trainer_council as tc
 
     class FakeOps:

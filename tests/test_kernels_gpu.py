@@ -210,38 +210,6 @@ def test_norm_fwd_bwd(ops, ref, C, adain_on, res_on, act, ups):
         check(d_adain, r_dad, 1e-4, 'norm bwd d_adain')
 
 
-@pytest.mark.parametrize('shape', [(2, 2, 12, 10, 64), (4, 8, 64, 64, 256), (3, 3, 32, 32, 128), (2, 5, 7, 9, 256), (1, 1, 256, 256, 64)])
-@pytest.mark.parametrize('adain_on,res_on,act,ups', [(False, False, 1, False), (True, True, 0, False), (True, False, 1, True)])
-def test_norm_single_launch_forms(ops, ref, shape, adain_on, res_on, act, ups):
-    """cg_norm_fused_fwd / cg_norm_fused_bwd (cooperative single-launch kernels with per-instance barriers) against the float64
-    reference AND against the two- / three-kernel forms they replace; shapes cover one round, several rounds (instances that do not
-    fit the L2 budget at once), odd sizes with empty pixel slices, and a single large instance split over every CTA."""
-    G, B, H, W, C = shape
-    y = rnd(G, B, H, W, C, seed=1, scale=2.0) + 0.5
-    P = 4 * C + 16
-    off = 8
-    adain = rnd(G, B, P, seed=2) if adain_on else None
-    res = rnd(G, B, H, W, C, seed=3) if res_on else None
-    z, mean, rstd = ops.norm_fused_fwd(y, adain, off, res, act, ups)
-    rm, rr = ref.in_stats(d(y))
-    check(mean, rm, 2e-5, 'mean')
-    check(rstd, rr, 2e-5, 'rstd')
-    check(z, ref.norm_act_fwd(d(y), rm, rr, d(adain), off, d(res), act, ups), 3e-5, 'fused norm fwd')
-    m2, r2 = ops.in_stats(y)
-    check(z, ops.norm_act_fwd(y, m2, r2, adain, off, res, act, ups), 2e-5, 'fused vs two-kernel fwd')
-    dz = rnd(*z.shape, seed=4)
-    d_adain = ops.zeros(G, B, P) if adain_on else None
-    dy = ops.norm_fused_bwd(dz, y, mean, rstd, adain, off, act, ups, d_adain)
-    r_dad = torch.zeros(G, B, P, dtype=torch.float64, device=DEV) if adain_on else None
-    rdy = ref.norm_act_bwd(d(dz), d(y), rm, rr, d(adain), off, act, ups, r_dad)
-    check(dy, rdy, 1e-4, 'fused norm bwd dy')
-    if adain_on:
-        check(d_adain, r_dad, 1e-4, 'fused norm bwd d_adain')
-    # run-to-run determinism (fixed reduction order, no atomics on data)
-    z2, _, _ = ops.norm_fused_fwd(y, adain, off, res, act, ups)
-    assert torch.equal(z, z2)
-
-
 def test_mask_head(ops, ref):
     G, B, H, W = 2, 2, 9, 7
     h = torch.tanh(rnd(G, B, H, W, 12, seed=1, scale=0.3))
