@@ -295,23 +295,29 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
         if (p.stats) {
             // instance-norm statistics of the raw convolution output, fused here instead of a second pass over y.  Every tile lies
             // inside one image (P*Q % 128 == 0); each warp reduces its 16 rows per column and writes one partial chunk.
+            // The 8 lanes of a column pair (lane % 4) hold (s0, s1, q0, q1) each and are summed in pairs at lane distance 4, 8,
+            // 16.  Transpose-reduce: at each level a lane keeps the half of its values that its lane bit selects and receives
+            // the partner's part of that half, so the 4 values take 4 shuffles instead of 12.  Every sum adds the same two
+            // operands as a plain butterfly (bits unchanged); lane l < 16 ends with element 2 * bit3 + bit2 of (s0, q0, s1, q1).
             const int tiles_per_img = pq / TC_BM;
             const int img = (mt * TC_BM) / pq;
             const int chunk = ((c * tiles_per_img + (mt - img * tiles_per_img)) << 3) + cw * 4 + warp4;
-            const long col0 = (long)(g * p.B + img) * p.Cout + nt * BN + cq;
+            const bool b2 = lane & 4, b3 = lane & 8;
+            float* st = p.stats + ((long)chunk * p.stats_gbc + (long)(g * p.B + img) * p.Cout + nt * BN + cq) * 2 + (b3 ? 2 : 0) + (b2 ? 1 : 0);
 #pragma unroll
             for (int j = 0; j < BN / 8; j++) {
-                float s0 = acc[4 * j] + acc[4 * j + 2], s1 = acc[4 * j + 1] + acc[4 * j + 3];
-                float q0 = acc[4 * j] * acc[4 * j] + acc[4 * j + 2] * acc[4 * j + 2];
-                float q1 = acc[4 * j + 1] * acc[4 * j + 1] + acc[4 * j + 3] * acc[4 * j + 3];
-#pragma unroll
-                for (int o = 4; o < 32; o <<= 1) {
-                    s0 += __shfl_xor_sync(0xffffffffu, s0, o);
-                    s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-                    q0 += __shfl_xor_sync(0xffffffffu, q0, o);
-                    q1 += __shfl_xor_sync(0xffffffffu, q1, o);
-                }
-                if (lane < 4) *reinterpret_cast<float4*>(p.stats + ((long)chunk * p.stats_gbc + col0 + 8 * j) * 2) = make_float4(s0, q0, s1, q1);
+                const float s0 = acc[4 * j] + acc[4 * j + 2], s1 = acc[4 * j + 1] + acc[4 * j + 3];
+                const float q0 = acc[4 * j] * acc[4 * j] + acc[4 * j + 2] * acc[4 * j + 2];
+                const float q1 = acc[4 * j + 1] * acc[4 * j + 1] + acc[4 * j + 3] * acc[4 * j + 3];
+                // level 4: keep (s0, s1) or (q0, q1)
+                const float k0 = b2 ? q0 : s0, k1 = b2 ? q1 : s1;
+                const float r0 = __shfl_xor_sync(0xffffffffu, b2 ? s0 : q0, 4), r1 = __shfl_xor_sync(0xffffffffu, b2 ? s1 : q1, 4);
+                const float x0 = k0 + r0, x1 = k1 + r1;
+                // level 8: keep column cq or cq + 1
+                float v = (b3 ? x1 : x0) + __shfl_xor_sync(0xffffffffu, b3 ? x0 : x1, 8);
+                // level 16
+                v += __shfl_xor_sync(0xffffffffu, v, 16);
+                if (lane < 16) st[16 * j] = v;
             }
         }
         // each row's 8-column group is written by four consecutive lanes: 32 contiguous bytes, one full sector
