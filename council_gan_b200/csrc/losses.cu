@@ -11,7 +11,9 @@
 //   total-loss assembly in gen_update                       trainer_council.py:392-451, 497-529, 559-634
 //   abs_beginning_end (recon_criterion_v2_color)            trainer_council.py:210-215, 477-495  (2 more launches per direction
 //                                                           while its weight gate is open)
+//   recon_x (recon_criterion of the within-domain decode)   trainer_council.py:339-345, 455-459
 #include "common.cuh"
+#include "mask_head.cuh"
 
 namespace cg {
 
@@ -471,6 +473,61 @@ __global__ void __launch_bounds__(L1_THREADS) latent_l1_kernel(const float* __re
     if (threadIdx.x == 0) *counter = 0u;
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// gen_update, image reconstruction (recon_x_w, trainer_council.py:339-345, 455-459): x_recon = the attention-mask composite of the
+// other direction's decoder head over the source image x; recon_criterion = mean |x_recon - x| over the 3 live lanes.  x_recon
+// feeds only this loss, so it is never written: pass 1 reduces the sums, the backward recomputes the composite (mask_head.cuh).
+// ---------------------------------------------------------------------------------------------------------------
+// pass 1: block (chunk, g) sums |x_recon - x| over GL_PIX pixels in float, the last block adds the chunks in double, in chunk order
+// (the convention of abs_be_fwd_kernel).  h [G][npix][12] (tanh output of the last head layer), x [npix][4] shared; part: float
+// [nchunks][G].
+__global__ void __launch_bounds__(256) recon_head_fwd_kernel(const float* __restrict__ h, const float* __restrict__ x, float* __restrict__ sums,
+                                                             float* __restrict__ part, unsigned int* __restrict__ counter, int G, long npix,
+                                                             int nchunks) {
+    pdl_trigger();
+    pdl_wait();
+    __shared__ float sm[32];
+    const int g = blockIdx.x % G, chunk = blockIdx.x / G;
+    const long p0 = (long)chunk * GL_PIX, p1 = min(npix, p0 + GL_PIX);
+    const float* hg = h + (long)g * npix * 12;
+    float v[1] = {0.f};
+    for (long px = p0 + threadIdx.x; px < p1; px += blockDim.x) {
+        MaskHeadPix p;
+        mask_composite(hg + px * 12, x + px * 4, p);
+        v[0] += fabsf(p.im[3][0] - p.im[0][0]) + fabsf(p.im[3][1] - p.im[0][1]) + fabsf(p.im[3][2] - p.im[0][2]);
+    }
+    block_sum<1>(v, sm);
+    if (threadIdx.x == 0) part[(long)chunk * G + g] = v[0];
+    if (!last_block_done(counter, gridDim.x)) return;
+    const int t = threadIdx.x;
+    if (t < G) {
+        const volatile float* vp = part;
+        double s = 0.0;
+        for (int c = 0; c < nchunks; c++) s += (double)vp[(long)c * G + t];
+        sums[t] = (float)s;
+    }
+    if (t == 0) *counter = 0u;
+}
+
+// backward: d(x_recon) = coef * sign(x_recon - x) (sign(0) = 0; coef = recon_x_w / numel of the GLOBAL minibatch) through the
+// composite and the head's tanh, as mask_head_bwd_kernel with d_mask = 0: dh_pre [G][npix][12]
+__global__ void __launch_bounds__(256) recon_head_bwd_kernel(const float* __restrict__ h, const float* __restrict__ x, float coef,
+                                                             float* __restrict__ dh_pre, long total, long npix) {
+    pdl_trigger();
+    pdl_wait();
+    const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    MaskHeadPix p;
+    mask_composite(h + i * 12, x + (i % npix) * 4, p);
+    float dim[3];
+#pragma unroll
+    for (int ch = 0; ch < 3; ch++) dim[ch] = coef * sgnf(p.im[3][ch] - p.im[0][ch]);
+    const float dm[3] = {0.f, 0.f, 0.f};
+    float out[12];
+    mask_head_grad(p, dim, dm, out);
+    store12(dh_pre + i * 12, out);
+}
+
 struct ReconTerms { double numel[CG_RECON_MAX_TERMS], w[CG_RECON_MAX_TERMS]; };
 
 // after the all-reduce: pub[k][g] = sums[k][g] / numel[k]; total[g] += sum_k w[k] * pub[k][g] through the double accumulator of
@@ -653,4 +710,25 @@ extern "C" int cg_recon_finalize(const float* sums, const double* host_numel, co
     }
     launch_k(recon_finalize_kernel, 1, 32, 0, ST, sums, t, nterm, G, total, ws_total64(ws), pub);
     return check_launch("recon_finalize");
+}
+
+extern "C" int cg_recon_head_fwd(const float* h, const float* x, float* sums, int G, int B, int HW, void* ws, size_t ws_bytes, void* stream) {
+    CG_REQUIRE(h && x && sums && G >= 1 && G <= CG_LOSS_MAX_G && B >= 1 && HW >= 1, "recon_head_fwd: G=%d B=%d HW=%d out of range", G, B,
+               HW);
+    const long npix = (long)B * HW;
+    const int nchunks = cdiv(npix, GL_PIX);
+    size_t need = 16 + CG_LOSS_MAX_G * 8 + (size_t)nchunks * G * 4;
+    if (need > ws_bytes) {
+        set_error("recon_head_fwd: workspace %zu < %zu bytes", ws_bytes, need);
+        return CG_ERR_WORKSPACE;
+    }
+    launch_k(recon_head_fwd_kernel, nchunks * G, 256, 0, ST, h, x, sums, ws_part(ws), ws_counter(ws), G, npix, nchunks);
+    return check_launch("recon_head_fwd");
+}
+
+extern "C" int cg_recon_head_bwd(const float* h, const float* x, float coef, float* dh_pre, int G, int B, int HW, void* stream) {
+    CG_REQUIRE(h && x && dh_pre && G >= 1 && B >= 1 && HW >= 1, "recon_head_bwd: G=%d B=%d HW=%d out of range", G, B, HW);
+    const long npix = (long)B * HW, total = npix * G;
+    launch_k(recon_head_bwd_kernel, cdiv(total, 256), 256, 0, ST, h, x, coef, dh_pre, total, npix);
+    return check_launch("recon_head_bwd");
 }

@@ -1,5 +1,6 @@
 // Image-space, loss and optimiser kernels (all HBM-bound; coalesced, vectorised where the layout allows).
 #include "common.cuh"
+#include "mask_head.cuh"
 
 namespace cg {
 
@@ -29,27 +30,17 @@ __device__ __forceinline__ void block_reduce(float (&v)[N], float* smem /* >= N*
     }
 }
 
-// ---- attention-mask head: Decoder_V2_atten.forward networks.py:398-407 -------------------------
-// h = tanh output of dec.model.9, 12 lanes: [o0 rgb | o1 rgb | o2 rgb | m0 m1 m2]
-// mask_k = (tanh(10*h[9+k])+1)/2;  im <- (1-mask_k)*im + mask_k*o_k, k = 0..2, starting from x_in
+// ---- attention-mask head: Decoder_V2_atten.forward networks.py:398-407 (compositing in mask_head.cuh) -----
 __global__ void mask_head_fwd_kernel(const float* __restrict__ h, const float* __restrict__ x_in, float* __restrict__ x_fake,
                                      float* __restrict__ mask, long total, long per_group) {
     pdl_trigger();
     pdl_wait();
     long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total) return;
-    const float* hp = h + i * 12;
-    float4 a = f4(hp), b = f4(hp + 4), c = f4(hp + 8);
-    float o[9] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w, c.x};
-    float mk[3] = {(tanhf(10.f * c.y) + 1.f) * 0.5f, (tanhf(10.f * c.z) + 1.f) * 0.5f, (tanhf(10.f * c.w) + 1.f) * 0.5f};
-    float4 xi = f4(x_in + (i % per_group) * 4);
-    float im[3] = {xi.x, xi.y, xi.z};
-#pragma unroll
-    for (int k = 0; k < 3; k++)
-#pragma unroll
-        for (int ch = 0; ch < 3; ch++) im[ch] = (1.f - mk[k]) * im[ch] + mk[k] * o[3 * k + ch];
-    reinterpret_cast<float4*>(x_fake)[i] = make_float4(im[0], im[1], im[2], 0.f);
-    reinterpret_cast<float4*>(mask)[i] = make_float4(mk[0], mk[1], mk[2], 0.f);
+    MaskHeadPix p;
+    mask_composite(h + i * 12, x_in + (i % per_group) * 4, p);
+    reinterpret_cast<float4*>(x_fake)[i] = make_float4(p.im[3][0], p.im[3][1], p.im[3][2], 0.f);
+    reinterpret_cast<float4*>(mask)[i] = make_float4(p.mk[0], p.mk[1], p.mk[2], 0.f);
 }
 
 __global__ void mask_head_bwd_kernel(const float* __restrict__ h, const float* __restrict__ x_in,
@@ -59,22 +50,8 @@ __global__ void mask_head_bwd_kernel(const float* __restrict__ h, const float* _
     pdl_wait();
     long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total) return;
-    const float* hp = h + i * 12;
-    float4 a = f4(hp), b = f4(hp + 4), c = f4(hp + 8);
-    float hv[12] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w, c.x, c.y, c.z, c.w};
-    float tk[3], mk[3];
-#pragma unroll
-    for (int k = 0; k < 3; k++) {
-        tk[k] = tanhf(10.f * hv[9 + k]);
-        mk[k] = (tk[k] + 1.f) * 0.5f;
-    }
-    float4 xi = f4(x_in + (i % per_group) * 4);
-    float im[4][3];
-    im[0][0] = xi.x; im[0][1] = xi.y; im[0][2] = xi.z;
-#pragma unroll
-    for (int k = 0; k < 3; k++)
-#pragma unroll
-        for (int ch = 0; ch < 3; ch++) im[k + 1][ch] = (1.f - mk[k]) * im[k][ch] + mk[k] * hv[3 * k + ch];
+    MaskHeadPix p;
+    mask_composite(h + i * 12, x_in + (i % per_group) * 4, p);
     float4 dx = f4(d_xfake + i * 4);
     float dim[3] = {dx.x, dx.y, dx.z};
     float dm[3] = {0.f, 0.f, 0.f};
@@ -82,25 +59,9 @@ __global__ void mask_head_bwd_kernel(const float* __restrict__ h, const float* _
         float4 d = f4(d_mask + i * 4);
         dm[0] = d.x; dm[1] = d.y; dm[2] = d.z;
     }
-    float dh[12];
-#pragma unroll
-    for (int k = 2; k >= 0; k--) {
-        float dmk = dm[k];
-#pragma unroll
-        for (int ch = 0; ch < 3; ch++) {
-            dh[3 * k + ch] = mk[k] * dim[ch];
-            dmk += dim[ch] * (hv[3 * k + ch] - im[k][ch]);
-            dim[ch] *= (1.f - mk[k]);
-        }
-        dh[9 + k] = dmk * 5.f * (1.f - tk[k] * tk[k]);  // d/dh (tanh(10h)+1)/2
-    }
     float out[12];
-#pragma unroll
-    for (int j = 0; j < 12; j++) out[j] = dh[j] * (1.f - hv[j] * hv[j]);  // through the layer's own tanh
-    float* op = dh_pre + i * 12;
-    *reinterpret_cast<float4*>(op) = make_float4(out[0], out[1], out[2], out[3]);
-    *reinterpret_cast<float4*>(op + 4) = make_float4(out[4], out[5], out[6], out[7]);
-    *reinterpret_cast<float4*>(op + 8) = make_float4(out[8], out[9], out[10], out[11]);
+    mask_head_grad(p, dim, dm, out);
+    store12(dh_pre + i * 12, out);
 }
 
 // ---- AvgPool2d(3, stride 2, pad 1, count_include_pad=False): networks.py:32,129 ------------------

@@ -57,14 +57,15 @@ class ParamBank:
             self.exp_avg_sq = ops.zeros(off)
         self.step = 0
 
-    def _view(self, buf, name):
+    def _view(self, buf, name, base=0):
+        """view of `name` in buf, a flat buffer laid out like grad[base:]"""
         # views are cached per (buffer object, name): ~430 lookups per step, each a slice + view (8 % of the host time of a step on the
         # launch-bound small configuration)
         hit = self._views.get((id(buf), name))
         if hit is not None and hit[0] is buf:
             return hit[1]
         off, shape, n = self.table[name]
-        v = buf[off:off + n].view((self.G,) + shape)
+        v = buf[off - base:off - base + n].view((self.G,) + shape)
         self._views[(id(buf), name)] = (buf, v)
         return v
 
@@ -278,8 +279,9 @@ class CouncilGen(_StackedNet):
         self.mlp = [LayerSpec('mlp.model.0.fc', self.mlp_dim, self.style_dim, 1, 1, 0, linear=True),
                     LayerSpec('mlp.model.1.fc', self.mlp_dim, self.mlp_dim, 1, 1, 0, linear=True),
                     LayerSpec('mlp.model.2.fc', self.n_adain, self.mlp_dim, 1, 1, 0, linear=True)]
-        # --- style encoder (networks.py:337-350): run by encode() / sample(), and in training only by the style reconstruction
-        # (recon_s_w != 0), the one term that gives it a gradient; otherwise its parameters are kept for the API / checkpoints
+        # --- style encoder (networks.py:337-350): run by encode() / sample(), and in training only by the style and image
+        # reconstructions (recon_s_w, recon_x_w != 0), the terms that give it a gradient; otherwise its parameters are kept for the API /
+        # checkpoints
         d = dim
         self.sty = [LayerSpec('enc_style.model.0.conv', d, input_dim, 7, 1, 3, lanes=img_lanes)]
         for i in range(2):
@@ -296,13 +298,14 @@ class CouncilGen(_StackedNet):
         # flat-buffer offset where the content encoder's parameters end: the decoder / head / MLP gradients [enc_end:] are
         # complete before the encoder backward starts, so data parallelism all-reduces them while it runs
         self.enc_end = self.bank.table[self.dec_res[0][0].wname][0] if self.dec_res else self.bank.table[self.head[0].wname][0]
-        # its own bank: gradients, Adam moments and step count only when recon_s_w trains it (torch's Adam starts a parameter's
-        # state at its first gradient, so this bank's step count can lag the generator's, e.g. after resuming with the term off)
+        # its own bank: gradients, Adam moments and step count only when recon_s_w or recon_x_w trains it (torch's Adam starts a
+        # parameter's state at its first gradient, so this bank's step count can lag the generator's, e.g. after resuming with the
+        # terms off)
         self.sty_bank = ParamBank(ops, G, [e for s in self.sty + [self.sty_out] for e in s.entries()],
-                                  trainable=hp.get('recon_s_w', 0) != 0)
+                                  trainable=hp.get('recon_s_w', 0) != 0 or hp.get('recon_x_w', 0) != 0)
         # biases feeding IN / AdaIN are mathematically dead (SURVEY.md 7.3-5): their gradient is exactly 0 here
         self.dead_bias = set(s.bname for s in live if s not in self.head and s not in self.mlp)
-        self._enc_grad2 = None
+        self._enc_grad2 = self._dec_grad2 = self._sty_grad2 = None
 
     @property
     def frozen(self):  # the style-encoder bank's earlier name
@@ -315,6 +318,27 @@ class CouncilGen(_StackedNet):
         if self._enc_grad2 is None:
             self._enc_grad2 = self.ops.zeros(self.enc_end)
         return self._enc_grad2
+
+    def decode_grad(self):
+        """Zero-initialised flat buffer laid out like bank.grad[enc_end:]: the decoder, head and MLP weight gradients of this
+        generator's second decoder pass in gen_update (recon_x: the other direction's image reconstruction), added to bank.grad after
+        the first pass's decoder backward.  The dead biases are never written, so they stay 0."""
+        if self._dec_grad2 is None:
+            self._dec_grad2 = self.ops.zeros(self.bank.total - self.enc_end)
+        return self._dec_grad2
+
+    def style_grad(self):
+        """Zero-initialised flat buffer laid out like sty_bank.grad: the style encoder's weight gradients of its second pass in
+        gen_update when it runs twice (recon_s on the other direction's translation, recon_x on the source image)."""
+        if self._sty_grad2 is None:
+            self._sty_grad2 = self.ops.zeros(self.sty_bank.total)
+        return self._sty_grad2
+
+    def _gv(self, grad, name):
+        """weight-gradient view of `name`: in bank.grad (grad None), decode_grad() or reencode_grad()"""
+        if grad is None:
+            return self.bank.g(name)
+        return self.bank._view(grad, name, self.enc_end if grad is self._dec_grad2 else 0)
 
     # -- state_dict plumbing -------------------------------------------------------------------------
     def _specs(self):
@@ -388,7 +412,7 @@ class CouncilGen(_StackedNet):
         x, y, mean, rstd = rec
         off = self.adain_off.get(s.key, 0)
         dy = ops.norm_act_bwd(dz, y, mean, rstd, adain, off, act, ups_out, d_adain)
-        ops.conv_wgrad(x, dy, self.bank.g(s.wname) if grad is None else self.bank._view(grad, s.wname), None, s.stride, s.pad)
+        ops.conv_wgrad(x, dy, self._gv(grad, s.wname), None, s.stride, s.pad)
         if not need_dx:
             return None
         return ops.conv_dgrad(dy, self.bank.p(s.wname), x.shape, s.stride, s.pad, addend=addend)
@@ -419,9 +443,12 @@ class CouncilGen(_StackedNet):
             saved.append(acts)
         return h.view(h.shape[0], h.shape[1], self.n_adain)
 
-    def decode(self, content, style, x_img, saved=None, sl=None):
-        """content [G,B,h,w,C], style [1,B,1,1,S], x_img [1,B,H,W,4] -> (x_fake, mask) [G,B,H,W,4]."""
+    def decode(self, content, style, x_img, saved=None, sl=None, recon_sums=None):
+        """content [G,B,h,w,C], style [1|G,B,1,1,S] (shared, or one code per member), x_img [1,B,H,W,4] -> (x_fake, mask) [G,B,H,W,4].
+        recon_sums [G]: end in the image reconstruction head instead (recon_x_w): recon_sums[g] = sum |x_recon - x_img| of member g,
+        the image and its mask are never written, and the result is None.  Needs saved."""
         ops = self.ops
+        assert recon_sums is None or saved is not None
         adain = self._mlp(style, saved, sl)
         x = content
         nres, nup = len(self.dec_res), len(self.dec_up)
@@ -448,6 +475,10 @@ class CouncilGen(_StackedNet):
             w, b = self._w(s, sl)
             x = ops.conv_fwd(x, w, b, 1, 0, act=ACT_RELU if li < 2 else ACT_TANH)
             acts.append(x)
+        if recon_sums is not None:
+            ops.recon_head_fwd(x, x_img, recon_sums)
+            saved.append((adain, acts, x_img))
+            return None
         x_fake, mask = ops.mask_head_fwd(x, x_img)
         if saved is not None:
             saved.append((adain, acts, x_img))
@@ -458,17 +489,31 @@ class CouncilGen(_StackedNet):
         """Fills ``self.bank.grad`` for every live parameter given d(loss)/d(x_fake), d(loss)/d(mask).
         on_decoder_done: called when grad[enc_end:] (decoder, head, MLP) is final, before the encoder backward.
         d_content: a further gradient of the content code (the recon_c target), added to what the decoder sends back."""
-        ops, bank = self.ops, self.bank
+        d, _ = self.decoder_backward(dec_saved, d_xfake, d_mask)
+        if on_decoder_done is not None:
+            on_decoder_done()
+        if d_content is not None:
+            self.ops.add_(d, d_content)
+        self.encode_backward(d, enc_saved)
+
+    def decoder_backward(self, dec_saved, d_xfake=None, d_mask=None, recon_coef=None, grad=None, want_dstyle=False):
+        """Backward of decode(..., saved=dec_saved) from d(loss)/d(x_fake), d(loss)/d(mask) -- or, for a pass that ended in the
+        reconstruction head, from recon_coef (d(x_recon) = recon_coef * sign(x_recon - x_img)).  Decoder, head and MLP weight gradients
+        go into bank.grad[enc_end:] (grad None) or decode_grad().  -> (d(content), d(style) [G,B,1,1,S] when want_dstyle else None)."""
+        ops = self.ops
         dec_saved = list(dec_saved)
         adain, acts, x_img = dec_saved.pop()
         mlp_acts = dec_saved.pop(0)
         d_adain = ops.empty(*adain.shape)  # every column is written by exactly one AdaIN layer's backward
-        # head: 1x1 convs with fused activations
-        d = ops.mask_head_bwd(acts[3], x_img, d_xfake, d_mask)  # grad w.r.t. pre-tanh output of head[2]
+        # head: 1x1 convs with fused activations; grad w.r.t. pre-tanh output of head[2]
+        if recon_coef is not None:
+            d = ops.recon_head_bwd(acts[3], x_img, recon_coef)
+        else:
+            d = ops.mask_head_bwd(acts[3], x_img, d_xfake, d_mask)
         for li in (2, 1, 0):
             s = self.head[li]
-            ops.conv_wgrad(acts[li], d, bank.g(s.wname), bank.g(s.bname), 1, 0)
-            d = ops.conv_dgrad(d, bank.p(s.wname), acts[li].shape, 1, 0,
+            ops.conv_wgrad(acts[li], d, self._gv(grad, s.wname), self._gv(grad, s.bname), 1, 0)
+            d = ops.conv_dgrad(d, self.bank.p(s.wname), acts[li].shape, 1, 0,
                                mask_src=acts[li] if li > 0 else None, mask_slope=0.0)
         # upsampling blocks, last to first
         recs = dec_saved  # one record per conv in forward order: dec_res (2*nr) then dec_up (2*nd)
@@ -476,30 +521,29 @@ class CouncilGen(_StackedNet):
         nup = len(self.dec_up)
         for u in range(nup - 1, -1, -1):
             a, b = self.dec_up[u]
-            d = self._conv_norm_bwd(d, b, recs[k], adain, d_adain, ACT_RELU, u + 1 < nup, None)
-            d = self._conv_norm_bwd(d, a, recs[k - 1], adain, d_adain, ACT_RELU, False, None)
+            d = self._conv_norm_bwd(d, b, recs[k], adain, d_adain, ACT_RELU, u + 1 < nup, None, grad=grad)
+            d = self._conv_norm_bwd(d, a, recs[k - 1], adain, d_adain, ACT_RELU, False, None, grad=grad)
             k -= 2
         if nup > 0:
             d = ops.upsample2x_bwd(d)  # the last residual block's output was written upsampled
         for blk in reversed(self.dec_res):
             d_out = d
-            d = self._conv_norm_bwd(d_out, blk[1], recs[k], adain, d_adain, ACT_NONE, False, None)
-            d = self._conv_norm_bwd(d, blk[0], recs[k - 1], adain, d_adain, ACT_RELU, False, d_out)
+            d = self._conv_norm_bwd(d_out, blk[1], recs[k], adain, d_adain, ACT_NONE, False, None, grad=grad)
+            d = self._conv_norm_bwd(d, blk[0], recs[k - 1], adain, d_adain, ACT_RELU, False, d_out, grad=grad)
             k -= 2
         assert k == -1
-        # MLP (gradients reach it through every AdaIN gamma/beta)
+        # MLP (gradients reach it through every AdaIN gamma/beta); layer 0's data gradient is d(style)
         dm = d_adain.view(d_adain.shape[0], d_adain.shape[1], 1, 1, self.n_adain)
+        d_style = None
         for li in (2, 1, 0):
             s = self.mlp[li]
             h_in, _ = mlp_acts[li]
-            ops.conv_wgrad(h_in, dm, bank.g(s.wname), bank.g(s.bname), 1, 0)
+            ops.conv_wgrad(h_in, dm, self._gv(grad, s.wname), self._gv(grad, s.bname), 1, 0)
             if li > 0:
-                dm = ops.conv_dgrad(dm, bank.p(s.wname), h_in.shape, 1, 0, mask_src=h_in, mask_slope=0.0)
-        if on_decoder_done is not None:
-            on_decoder_done()
-        if d_content is not None:
-            ops.add_(d, d_content)
-        self.encode_backward(d, enc_saved)
+                dm = ops.conv_dgrad(dm, self.bank.p(s.wname), h_in.shape, 1, 0, mask_src=h_in, mask_slope=0.0)
+            elif want_dstyle:
+                d_style = ops.conv_dgrad(dm, self.bank.p(s.wname), h_in.shape, 1, 0)
+        return d, d_style
 
     def encode_backward(self, d, enc_saved, grad=None, want_dx=False, addend=None):
         """Backward of encode(x, enc_saved) from d(content): weight gradients into bank.grad (or the flat buffer grad laid out like
@@ -530,7 +574,8 @@ class CouncilGen(_StackedNet):
     def style_encode(self, x, sl=None, saved=None):
         """StyleEncoder networks.py:337-353 (norm none, relu), all members (or member sl) at once:
         x [1|G,B,H,W,4] -> style codes [G,B,1,1,style_dim].  In training only the style reconstruction (recon_s_w) runs it, on the
-        other direction's translations; saved (a list) keeps what style_backward needs."""
+        other direction's translations, and the image reconstruction (recon_x_w), on the source images; saved (a list) keeps what
+        style_backward needs."""
         ops, sb = self.ops, self.sty_bank
 
         def wb(s):
@@ -551,18 +596,23 @@ class CouncilGen(_StackedNet):
             pooled = h.mean(dim=(2, 3), keepdim=True).contiguous()
         return ops.conv_fwd(pooled, *wb(self.sty_out), 1, 0)
 
-    def style_backward(self, d_s, saved, addend=None):
-        """Backward of style_encode(x, saved=saved) from d(style code) [G,B,1,1,S]: weight and bias gradients into sty_bank.grad;
-        returns d(x) [G,B,H,W,4] (+ addend)."""
+    def style_backward(self, d_s, saved, addend=None, want_dx=True, grad=None):
+        """Backward of style_encode(x, saved=saved) from d(style code) [G,B,1,1,S]: weight and bias gradients into sty_bank.grad (or
+        style_grad()); returns d(x) [G,B,H,W,4] (+ addend), or None without want_dx (x a real image: the 7x7 data gradient is skipped)."""
         ops, sb = self.ops, self.sty_bank
+
+        def gv(name):
+            return sb.g(name) if grad is None else sb._view(grad, name)
         acts, pooled = saved
         s = self.sty_out
-        ops.conv_wgrad(pooled, d_s, sb.g(s.wname), sb.g(s.bname), 1, 0)
+        ops.conv_wgrad(pooled, d_s, gv(s.wname), gv(s.bname), 1, 0)
         d = ops.conv_dgrad(d_s, sb.p(s.wname), pooled.shape, 1, 0)
         d = ops.global_avgpool_bwd(d, acts[-1])  # gated by the last layer's ReLU
         for li in range(len(self.sty) - 1, -1, -1):
             s = self.sty[li]
-            ops.conv_wgrad(acts[li], d, sb.g(s.wname), sb.g(s.bname), s.stride, s.pad)
+            ops.conv_wgrad(acts[li], d, gv(s.wname), gv(s.bname), s.stride, s.pad)
+            if li == 0 and not want_dx:
+                return None
             d = ops.conv_dgrad(d, sb.p(s.wname), acts[li].shape, s.stride, s.pad, addend=addend if li == 0 else None,
                                mask_src=acts[li] if li > 0 else None, mask_slope=0.0)
         return d

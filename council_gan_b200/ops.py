@@ -87,6 +87,8 @@ _SIGS = {
     'cg_latent_l1': (C.c_int, [_fp, _fp, C.c_int, _fp, _fp, C.c_float, C.c_int, _fp, C.c_int, C.c_long, _fp, C.c_size_t, _fp]),
     'cg_recon_finalize': (C.c_int, [_fp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int, C.c_int, _fp, _fp, _fp, C.c_size_t,
                                     _fp]),
+    'cg_recon_head_fwd': (C.c_int, [_fp, _fp, _fp, C.c_int, C.c_int, C.c_int, _fp, C.c_size_t, _fp]),
+    'cg_recon_head_bwd': (C.c_int, [_fp, _fp, C.c_float, _fp, C.c_int, C.c_int, C.c_int, _fp]),
     'cg_global_avgpool_fwd': (C.c_int, [_fp, _fp, C.c_int, C.c_int, C.c_int, _fp]),
     'cg_global_avgpool_bwd': (C.c_int, [_fp, _fp, _fp, C.c_int, C.c_int, C.c_int, C.c_int, _fp]),
     'cg_loss_workspace_bytes': (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int]),
@@ -652,6 +654,29 @@ class CudaOps:
         ws = self._loss_scratch(G)  # never grows the scratch: a new buffer would drop the accumulator gen_loss_bwd left in it
         self._ck(self.lib.cg_recon_finalize(_p(sums), (C.c_double * K)(*numel), (C.c_double * K)(*weights), K, G, _p(total), _p(pub),
                                             _p(ws), ws.numel(), self._stream()), 'cg_recon_finalize')
+
+    def recon_head_fwd(self, h, x_in, sums):
+        """recon_x pass 1: sums[g] = sum |x_recon - x_in| over the 3 live lanes of member g on this rank, x_recon the mask_head_fwd
+        composite of h [G,B,H,W,12] (tanh output of the last head layer) over x_in [1,B,H,W,4].  x_recon is never written.  ONE launch."""
+        self._chk(h, x_in, sums)
+        G, B, H, W, _ = h.shape
+        assert tuple(x_in.shape) == (1, B, H, W, 4) and sums.numel() == G
+        ws = self._loss_scratch(G, B, H, W)
+        self._timed_raw('hbm:recon_head_fwd G%d B%d %dx%d' % (G, B, H, W), 4.0 * (h.numel() + x_in.numel()),
+                        lambda: self._ck(self.lib.cg_recon_head_fwd(_p(h), _p(x_in), _p(sums), G, B, H * W, _p(ws), ws.numel(),
+                                                                    self._stream()), 'cg_recon_head_fwd'))
+
+    def recon_head_bwd(self, h, x_in, coef):
+        """recon_x backward: the gradient w.r.t. the pre-tanh head output [G,B,H,W,12] for d(x_recon) = coef * sign(x_recon - x_in)
+        (sign(0) = 0) and no mask gradient, the composite recomputed.  ONE launch."""
+        self._chk(h, x_in)
+        G, B, H, W, _ = h.shape
+        assert tuple(x_in.shape) == (1, B, H, W, 4)
+        dh = self.empty(G, B, H, W, 12)
+        self._timed_raw('hbm:recon_head_bwd G%d B%d %dx%d' % (G, B, H, W), 4.0 * (2 * h.numel() + x_in.numel()),
+                        lambda: self._ck(self.lib.cg_recon_head_bwd(_p(h), _p(x_in), float(coef), _p(dh), G, B, H * W, self._stream()),
+                                         'cg_recon_head_bwd'))
+        return dh
 
     # -- input pipeline (council_gan_b200/data.py) ------------------------------------------------------
     def aug_color(self, pix, desc, opcode, param, B, max_pixels, any_contrast):

@@ -36,8 +36,15 @@ What is different underneath (GPU-first, see DESIGN.md):
     content gradient, and the content encoder's weight gradients of its two passes are summed.  recon_s_w is the only term
     that trains the style encoder; its bank then has its own Adam state.  With both weights 0 (the shipped configs) nothing
     of it runs.
-Paths outside the live configuration space of the reference's three configs (recon_x / recon_x_cyc / vgg / council_abs
-losses, nsgan/RaHinge, do_my_style, gray-scale D, random D/G pairing) raise NotImplementedError.
+  * recon_x_w (:339-345, 455-459, the within-domain image reconstruction; both directions required): each source image is
+    style-encoded by its own generator, and the other direction's generator decodes (own content code, own style code, source
+    image) through a reconstruction head that composites like the mask head but writes only the per-member sums of |x_recon - x|
+    (one more pair of rows in the scalar all-reduce).  Its backward runs with the re-encode backward: the other generator's
+    decoder, head and MLP gradients go into a scratch added after that generator's own decoder backward, d(content) joins the
+    content gradient, and d(style) trains this generator's style encoder on the source image (summed with recon_s's pass when both
+    are on).  The reconstruction's mask takes no loss.  With recon_x_w 0 (the shipped configs) nothing of it runs.
+Paths outside the live configuration space of the reference's three configs (recon_x_cyc / vgg / council_abs losses,
+nsgan/RaHinge, do_my_style, gray-scale D, random D/G pairing) raise NotImplementedError.
 """
 from __future__ import annotations
 
@@ -226,11 +233,11 @@ class Council_Trainer(nn.Module):
     # ------------------------------------------------------------------------------------------------
     @staticmethod
     def _check_supported(hp):
-        bad = [k for k in ('recon_x_w', 'recon_x_cyc_w', 'vgg_w', 'council_abs_w') if hp.get(k, 0) != 0]
+        bad = [k for k in ('recon_x_cyc_w', 'vgg_w', 'council_abs_w') if hp.get(k, 0) != 0]
         if bad:
             raise NotImplementedError('loss terms %s are not on the accelerated training path' % bad)
-        if (hp.get('recon_c_w', 0) != 0 or hp.get('recon_s_w', 0) != 0) and not (hp['do_a2b'] and hp['do_b2a']):
-            raise NotImplementedError('recon_c_w / recon_s_w re-encode each translation with the other direction\'s generator, so '
+        if any(hp.get(k, 0) != 0 for k in ('recon_x_w', 'recon_c_w', 'recon_s_w')) and not (hp['do_a2b'] and hp['do_b2a']):
+            raise NotImplementedError('recon_x_w / recon_c_w / recon_s_w decode or re-encode with the other direction\'s generator, so '
                                       'they need do_a2b and do_b2a (with one direction the reference fails with an IndexError)')
         if hp['dis']['gan_type'] != 'lsgan':
             assert 0, "Unsupported GAN type: {}".format(hp['dis']['gan_type'])
@@ -565,12 +572,11 @@ class Council_Trainer(nn.Module):
         center, eps = float(fl['mask_zero_or_one_center']), float(fl['mask_zero_or_one_epsilon'])
         be_w = self._abs_beginning_end_weights(hp, iterations)
         be_on = bool(be_w)
-        # latent reconstruction (:359-369, 460-469): the terms in the reference's list order, as (kind, domain, weight); the
-        # translation of direction d is re-encoded by the other direction's generator
-        recon = ([('s', 'a', hp['recon_s_w']), ('s', 'b', hp['recon_s_w'])] if hp['recon_s_w'] != 0 else []) + \
-                ([('c', 'a', hp['recon_c_w']), ('c', 'b', hp['recon_c_w'])] if hp['recon_c_w'] != 0 else [])
-        if hp['recon_s_w'] != 0 and not all(self._nets['gen_' + d].sty_bank.trainable for d in self._dirs):
-            raise NotImplementedError('recon_s_w trains the style encoder: it must be non-zero when the trainer is built')
+        # image and latent reconstruction (:339-345, 359-369, 455-469): the terms in the reference's order, as (kind, domain, weight);
+        # x: the source of domain dom decoded by the other direction's generator, s / c: the translation of direction d re-encoded
+        recon = [(kind, dom, hp['recon_%s_w' % kind]) for kind in ('x', 's', 'c') if hp['recon_%s_w' % kind] != 0 for dom in ('a', 'b')]
+        if (hp['recon_s_w'] != 0 or hp['recon_x_w'] != 0) and not all(self._nets['gen_' + d].sty_bank.trainable for d in self._dirs):
+            raise NotImplementedError('recon_s_w / recon_x_w train the style encoder: they must be non-zero when the trainer is built')
 
         # ---- forward of every direction; pass 1 of the loss (all reductions, one launch per direction) -----------
         fw = {}
@@ -611,7 +617,7 @@ class Council_Trainer(nn.Module):
             if be_on:
                 ops.abs_beginning_end_fwd(x_fake, src, be_sums[di])
             if recon:
-                rec['c'] = c
+                rec['c'], rec['src'] = c, src
             fw[d] = rec
         if recon:
             recon_numel = self._recon_forward(fw, s, recon, rc_sums)
@@ -629,6 +635,13 @@ class Council_Trainer(nn.Module):
             be_weights = [float(w) for w in be_w] + [0.0] * (N - len(be_w))  # 0: this member's gate is closed
         matching = bool(self.do_w_loss_matching)
         data_parallel = self.world > 1
+        recon_x_on = hp['recon_x_w'] != 0
+
+        def decoder_done(g):  # grad[enc_end:] of g is final once recon_x's pass through its decoder is added
+            if recon_x_on:
+                ops.add_(g.bank.grad[g.enc_end:], g.decode_grad())
+            if data_parallel:
+                self._reduce_async('gen', g, g.enc_end, None)
         for di, d in enumerate(self._dirs):
             rec = fw[d]
             gen = self._nets['gen_' + d]
@@ -665,9 +678,9 @@ class Council_Trainer(nn.Module):
                 ops.abs_beginning_end_bwd(rec['x_fake'], self._src(d, img_a, img_b), be_sums[di], hpd['numel'], be_weights, total,
                                           be_pub[di], d_x)
             gen.backward(d_x, d_mask, rec['enc'], rec['dec'],
-                         on_decoder_done=(lambda g=gen: self._reduce_async('gen', g, g.enc_end, None))
-                         if data_parallel else None, d_content=rec.get('d_c'))
-            if 'd_c' in rec:  # the content encoder ran twice: add the re-encode pass's weight gradients
+                         on_decoder_done=(lambda g=gen: decoder_done(g)) if recon_x_on or data_parallel else None,
+                         d_content=rec.get('d_c'))
+            if hp['recon_c_w'] != 0:  # the content encoder ran twice: add the re-encode pass's weight gradients
                 ops.add_(gen.bank.grad[:gen.enc_end], gen.reencode_grad())
             if data_parallel:
                 self._reduce_async('gen', gen, 0, gen.enc_end)  # encoder bucket; the decoder bucket went out during the encoder backward
@@ -702,8 +715,8 @@ class Council_Trainer(nn.Module):
         if be_w is not None:  # :477-484: one entry per member whose gate was open, the int 0 for an inactive direction
             for d, name in (('a2b', 'loss_gen_beginning_end_a_ab_s'), ('b2a', 'loss_gen_beginning_end_b_ba_s')):
                 setattr(self, name, [be_pub[self._dirs.index(d), i] for i in range(len(be_w))] if d in fw else [0] * len(be_w))
-        if recon:  # :310-313, :460-469: one entry per member, [] for a term whose weight is 0
-            for kind in ('s', 'c'):
+        if recon:  # :308-313, :455-469: one entry per member, [] for a term whose weight is 0
+            for kind in ('x', 's', 'c'):
                 for dom in ('a', 'b'):
                     setattr(self, 'loss_gen_recon_%s_%s_s' % (kind, dom), [])
             for k, (kind, dom, _) in enumerate(recon):
@@ -711,13 +724,25 @@ class Council_Trainer(nn.Module):
         self._last_fw = {d: {'x_fake': fw[d]['x_fake'], 'mask': fw[d]['mask']} for d in self._dirs}
 
     def _recon_forward(self, fw, s, recon, sums):
-        """Re-encode each translation with the other direction's generator (:359-369), keeping activations for the backward, and
-        evaluate the latent reconstruction terms: sums[k] = this rank's sum |recon - target| of term k, written together with the
-        gradients (they do not depend on the loss value).  -> numel of each term over the GLOBAL minibatch."""
+        """The reconstruction passes, keeping activations for the backward, and their terms: sums[k] = this rank's sum |recon - target|
+        of term k.  recon_x (:339-345): the source of direction d, style-encoded by its own generator, decoded by the other one through
+        the reconstruction head.  recon_s / recon_c (:359-369): each translation re-encoded by the other direction's generator; their
+        gradients are written together with the sums (they do not depend on the loss value).  -> numel of each term over the GLOBAL
+        minibatch."""
         ops = self.ops
         other = {'a2b': 'b2a', 'b2a': 'a2b'}
         numel = []
         for k, (kind, dom, w) in enumerate(recon):
+            if kind == 'x':  # x_a_recon = gen_b2a.decode(c_a, s_a', x_a): mean |x_recon - x| over B x 3 x H x W
+                d = 'a2b' if dom == 'a' else 'b2a'
+                rec = fw[d]
+                rec['sx_saved'], rec['x_dec_saved'] = [], []
+                s_prime = self._nets['gen_' + d].style_encode(rec['src'], saved=rec['sx_saved'])
+                self._nets['gen_' + other[d]].decode(rec['c'], s_prime, rec['src'], rec['x_dec_saved'], recon_sums=sums[k])
+                n = rec['B'] * 3 * rec['H'] * rec['W'] * self.world
+                rec['x_coef'] = float(w) / n
+                numel.append(float(n))
+                continue
             # recon_c_a / recon_s_b come from re-encoding x_ab (direction a2b), recon_c_b / recon_s_a from x_ba
             d = ('a2b' if dom == 'a' else 'b2a') if kind == 'c' else ('a2b' if dom == 'b' else 'b2a')
             rec = fw[d]
@@ -738,22 +763,40 @@ class Council_Trainer(nn.Module):
         return numel
 
     def _recon_backward(self, fw, recon):
-        """Backward of both re-encodes, before either generator's own backward: the other generator's style-encoder gradients (then
-        queued for its all-reduce) and content-encoder gradients (into its reencode_grad() buffer), and d(recon) / d(x_fake) of every
-        direction that has a term."""
+        """Backward of the reconstruction passes, before either generator's own backward.  recon_x: the other generator's decoder
+        (weight gradients into its decode_grad() buffer), its d(content) joining the content gradient of the direction and its d(style)
+        training this generator's style encoder without a data gradient to the image.  recon_s / recon_c: the other generator's
+        style-encoder and content-encoder gradients (the latter into its reencode_grad() buffer).  A style encoder that ran twice sums
+        its two passes, and each style bank's all-reduce is queued once, after all of its contributions.  -> d(recon) / d(x_fake) of
+        every direction that has a re-encode term."""
+        ops = self.ops
         other = {'a2b': 'b2a', 'b2a': 'a2b'}
+        kinds = set(kind for kind, _, _ in recon)
+        both_styles = 'x' in kinds and 's' in kinds
         d_x = {}
         for d in self._dirs:
             rec = fw[d]
-            gen_o = self._nets['gen_' + other[d]]
+            gen_d, gen_o = self._nets['gen_' + d], self._nets['gen_' + other[d]]
+            if 'x_dec_saved' in rec:
+                d_c, d_s = gen_o.decoder_backward(rec['x_dec_saved'], recon_coef=rec['x_coef'], grad=gen_o.decode_grad(), want_dstyle=True)
+                if 'd_c' in rec:
+                    ops.add_(rec['d_c'], d_c)
+                else:
+                    rec['d_c'] = d_c
+                gen_d.style_backward(d_s, rec['sx_saved'], want_dx=False, grad=gen_d.style_grad() if both_styles else None)
             dx = None
             if 's_saved' in rec:
                 dx = gen_o.style_backward(rec['d_s_rec'], rec['s_saved'])
-                self._reduce_async('gen', gen_o, bank=gen_o.sty_bank)
             if 'c_saved' in rec:
                 dx = gen_o.encode_backward(rec['d_c_rec'], rec['c_saved'], grad=gen_o.reencode_grad(), want_dx=True, addend=dx)
             if dx is not None:
                 d_x[d] = dx
+        if kinds & {'x', 's'}:
+            for d in self._dirs:
+                gen = self._nets['gen_' + d]
+                if both_styles:
+                    ops.add_(gen.sty_bank.grad, gen.style_grad())
+                self._reduce_async('gen', gen, bank=gen.sty_bank)
         return d_x
 
     # ==================================================================================================

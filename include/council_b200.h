@@ -238,12 +238,19 @@ int cg_abs_beginning_end_bwd(const float* x_fake, const float* x, const float* s
  * coef = w / numel of the GLOBAL minibatch.  db needs a per-member b. */
 int cg_latent_l1(const float* a, const float* b, int b_shared, float* da, float* db, float coef, int accumulate, float* sums,
                  int G, long n, void* ws, size_t ws_bytes, void* stream);
-#define CG_RECON_MAX_TERMS 4
+#define CG_RECON_MAX_TERMS 6
 /* after the all-reduce of sums[nterm][G]: pub[k][g] = sums[k][g] / host_numel[k]; total[g] += sum_k host_weight[k] * pub[k][g]
  * through the double accumulator cg_gen_loss_bwd keeps in the same workspace (so it must follow the cg_gen_loss_bwd calls of
  * this update on that workspace and stream).  host_numel / host_weight (host memory) are passed by value. */
 int cg_recon_finalize(const float* sums, const double* host_numel, const double* host_weight, int nterm, int G, float* total,
                       float* pub, void* ws, size_t ws_bytes, void* stream);
+/* image reconstruction (recon_x_w, trainer_council.py:339-345, 455-459): h[G][B][HW][12] = tanh output of the last head layer of
+ * the other direction's decoder, x[B][HW][4] the shared source image; x_recon = the cg_mask_head_fwd composite, never written.
+ * fwd: sums[g] = sum |x_recon - x| over the 3 live lanes of member g on this rank (float per block of 2048 pixels, blocks added in
+ * double in a fixed order).  bwd: dh_pre[G][B][HW][12] = cg_mask_head_bwd's result for d_xfake = coef * sign(x_recon - x)
+ * (sign(0) = 0) and d_mask = 0, the composite recomputed bit for bit. */
+int cg_recon_head_fwd(const float* h, const float* x, float* sums, int G, int B, int HW, void* ws, size_t ws_bytes, void* stream);
+int cg_recon_head_bwd(const float* h, const float* x, float coef, float* dh_pre, int G, int B, int HW, void* stream);
 size_t cg_loss_workspace_bytes(int G, int B, int H, int W);
 
 /* plumbing: p[0:bytes] = 0 on `stream` (cudaMemsetAsync; keeps framework fill kernels out of the launch list) */
