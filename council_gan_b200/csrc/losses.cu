@@ -12,6 +12,8 @@
 //   abs_beginning_end (recon_criterion_v2_color)            trainer_council.py:210-215, 477-495  (2 more launches per direction
 //                                                           while its weight gate is open)
 //   recon_x (recon_criterion of the within-domain decode)   trainer_council.py:339-345, 455-459
+//   council_abs_w (council_basic_criterion_*)               trainer_council.py:224-228, 595-619  (2 more launches per direction
+//                                                           while the council gate is open)
 #include "common.cuh"
 #include "mask_head.cuh"
 
@@ -411,6 +413,90 @@ __global__ void __launch_bounds__(256) abs_be_bwd_kernel(const float* __restrict
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// gen_update, council abs loss (council_abs_w, trainer_council.py:224-228, 595-619): member g's translation against the detached
+// translation of its peer p[g], mean |x_g - x_p| over the 3 live lanes (colour) or mean |sum_c x_g - sum_c x_p| (gray scale)
+// ---------------------------------------------------------------------------------------------------------------
+struct CouncilPeers { int p[CG_LOSS_MAX_G]; };  // host-drawn peers, passed by value
+
+// pr.p[g] without a dynamic index into the parameter struct (which would copy it to the stack)
+__device__ __forceinline__ int peer_of(const CouncilPeers& pr, int g) {
+    int p = 0;
+#pragma unroll
+    for (int k = 0; k < CG_LOSS_MAX_G; k++) p = k == g ? pr.p[k] : p;
+    return p;
+}
+
+// |x_g - x_p| of one pixel (colour: 3 lanes; gray: the channel sums, as torch.sum(x, 1) - torch.sum(y, 1))
+__device__ __forceinline__ float council_abs_pix(const float4 a, const float4 b, int gray) {
+    return gray ? fabsf((a.x + a.y + a.z) - (b.x + b.y + b.z)) : fabsf(a.x - b.x) + fabsf(a.y - b.y) + fabsf(a.z - b.z);
+}
+
+// pass 1: block (chunk, g) sums over GL_PIX pixels in float, the last block adds the chunks in double, in chunk order (the convention
+// of abs_be_fwd_kernel).  part: float [nchunks][G].
+__global__ void __launch_bounds__(256) council_abs_fwd_kernel(const float* __restrict__ x_fake, const CouncilPeers pr, int gray,
+                                                              float* __restrict__ sums, float* __restrict__ part,
+                                                              unsigned int* __restrict__ counter, int G, long npix, int nchunks) {
+    pdl_trigger();
+    pdl_wait();
+    __shared__ float sm[32];
+    const int g = blockIdx.x % G, chunk = blockIdx.x / G;
+    const long p0 = (long)chunk * GL_PIX, p1 = min(npix, p0 + GL_PIX);
+    const float* xg = x_fake + (long)g * npix * 4;
+    const float* xp = x_fake + (long)peer_of(pr, g) * npix * 4;
+    float v[1] = {0.f};
+    for (long px = p0 + threadIdx.x; px < p1; px += blockDim.x) v[0] += council_abs_pix(ld4(xg + px * 4), ld4(xp + px * 4), gray);
+    block_sum<1>(v, sm);
+    if (threadIdx.x == 0) part[(long)chunk * G + g] = v[0];
+    if (!last_block_done(counter, gridDim.x)) return;
+    const int t = threadIdx.x;
+    if (t < G) {
+        const volatile float* vp = part;
+        double s = 0.0;
+        for (int c = 0; c < nchunks; c++) s += (double)vp[(long)c * G + t];
+        sums[t] = (float)s;
+    }
+    if (t == 0) *counter = 0u;
+}
+
+// pass 2 (sums summed over ranks, numel of the GLOBAL minibatch): block 0 publishes the weighted term pub[g] = w * sums[g] / numel and
+// adds it to the double accumulator of the direction totals; a grid-stride pass adds w / numel * sign(d) to d_x on lanes 0..2 (gray:
+// the sign of the channel-sum difference on all three), sign(0) = 0.  The peer's image takes no gradient.
+__global__ void __launch_bounds__(256) council_abs_bwd_kernel(const float* __restrict__ x_fake, const CouncilPeers pr, int gray,
+                                                              const float* __restrict__ sums, double numel, double w, int G, long npix,
+                                                              float* __restrict__ total, double* __restrict__ total64,
+                                                              float* __restrict__ pub, float* __restrict__ d_x) {
+    pdl_trigger();
+    pdl_wait();
+    __shared__ long s_off[CG_LOSS_MAX_G];  // pixel offset of member g's peer
+    if ((int)threadIdx.x < G) {
+        const int g = threadIdx.x;
+        s_off[g] = (long)(peer_of(pr, g) - g) * npix;
+        if (blockIdx.x == 0) {
+            const double term = w * ((double)sums[g] / numel);
+            pub[g] = (float)term;
+            const double t64 = total64[g] + term;
+            total64[g] = t64;
+            total[g] = (float)t64;
+        }
+    }
+    __syncthreads();
+    const float c = (float)(w / numel);
+    const long total_px = npix * G, stride = (long)gridDim.x * blockDim.x;
+    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total_px; i += stride) {
+        const int g = (int)(i / npix);
+        const float4 a = ld4(x_fake + i * 4), b = ld4(x_fake + (i + s_off[g]) * 4);
+        float4 o = reinterpret_cast<const float4*>(d_x)[i];
+        if (gray) {
+            const float s = c * sgnf((a.x + a.y + a.z) - (b.x + b.y + b.z));
+            o.x += s; o.y += s; o.z += s;
+        } else {
+            o.x += c * sgnf(a.x - b.x); o.y += c * sgnf(a.y - b.y); o.z += c * sgnf(a.z - b.z);
+        }
+        reinterpret_cast<float4*>(d_x)[i] = o;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // gen_update, latent reconstruction (recon_c_w / recon_s_w, trainer_council.py:359-369, 460-469): recon_criterion = mean |a - b|
 // of a re-encoded content / style code a against its target b
 // ---------------------------------------------------------------------------------------------------------------
@@ -670,6 +756,49 @@ extern "C" int cg_abs_beginning_end_bwd(const float* x_fake, const float* x, con
     if (blocks > cap) blocks = cap;
     launch_k(abs_be_bwd_kernel, blocks, 256, 0, ST, x_fake, x, sums, numel, wt, G, npix, total, ws_total64(ws), pub, d_x);
     return check_launch("abs_beginning_end_bwd");
+}
+
+static int council_peers(const int32_t* host_peer, int G, CouncilPeers& pr, const char* who) {
+    CG_REQUIRE(host_peer && G >= 1 && G <= CG_LOSS_MAX_G, "%s: G=%d out of range", who, G);
+    for (int g = 0; g < G; g++) {
+        CG_REQUIRE(host_peer[g] >= 0 && host_peer[g] < G && host_peer[g] != g, "%s: peer %d of member %d is not another member", who,
+                   host_peer[g], g);
+        pr.p[g] = host_peer[g];
+    }
+    return CG_OK;
+}
+
+extern "C" int cg_council_abs_fwd(const float* x_fake, const int32_t* host_peer, int gray, float* sums, int G, int B, int H, int W,
+                                  void* ws, size_t ws_bytes, void* stream) {
+    CouncilPeers pr = {};
+    if (int rc = council_peers(host_peer, G, pr, "council_abs_fwd")) return rc;
+    CG_REQUIRE(x_fake && sums && B >= 1 && H >= 1 && W >= 1, "council_abs_fwd: B=%d H=%d W=%d out of range", B, H, W);
+    const long npix = (long)B * H * W;
+    const int nchunks = cdiv(npix, GL_PIX);
+    size_t need = 16 + CG_LOSS_MAX_G * 8 + (size_t)nchunks * G * 4;
+    if (need > ws_bytes) {
+        set_error("council_abs_fwd: workspace %zu < %zu bytes", ws_bytes, need);
+        return CG_ERR_WORKSPACE;
+    }
+    launch_k(council_abs_fwd_kernel, nchunks * G, 256, 0, ST, x_fake, pr, gray, sums, ws_part(ws), ws_counter(ws), G, npix, nchunks);
+    return check_launch("council_abs_fwd");
+}
+
+extern "C" int cg_council_abs_bwd(const float* x_fake, const int32_t* host_peer, int gray, const float* sums, double numel, double w,
+                                  float* total, float* pub, float* d_x, int G, int B, int H, int W, void* ws, size_t ws_bytes,
+                                  void* stream) {
+    CouncilPeers pr = {};
+    if (int rc = council_peers(host_peer, G, pr, "council_abs_bwd")) return rc;
+    CG_REQUIRE(x_fake && sums && total && pub && d_x && B >= 1 && H >= 1 && W >= 1, "council_abs_bwd: B=%d H=%d W=%d out of range", B,
+               H, W);
+    CG_REQUIRE(numel > 0, "council_abs_bwd: numel must be positive");
+    CG_REQUIRE(ws_bytes >= 16 + CG_LOSS_MAX_G * 8, "council_abs_bwd: workspace too small");
+    const long npix = (long)B * H * W;
+    int blocks = cdiv(npix * G, 256);
+    const int cap = 8 * (tc_sm_count() > 0 ? tc_sm_count() : 1);
+    if (blocks > cap) blocks = cap;
+    launch_k(council_abs_bwd_kernel, blocks, 256, 0, ST, x_fake, pr, gray, sums, numel, w, G, npix, total, ws_total64(ws), pub, d_x);
+    return check_launch("council_abs_bwd");
 }
 
 static int latent_l1_blocks(long n) {

@@ -84,6 +84,9 @@ _SIGS = {
     'cg_abs_beginning_end_fwd': (C.c_int, [_fp, _fp, _fp] + [C.c_int] * 4 + [_fp, C.c_size_t, _fp]),
     'cg_abs_beginning_end_bwd': (C.c_int, [_fp, _fp, _fp, C.c_double, C.POINTER(C.c_double), _fp, _fp, _fp] + [C.c_int] * 4 +
                                  [_fp, C.c_size_t, _fp]),
+    'cg_council_abs_fwd': (C.c_int, [_fp, C.POINTER(C.c_int32), C.c_int, _fp] + [C.c_int] * 4 + [_fp, C.c_size_t, _fp]),
+    'cg_council_abs_bwd': (C.c_int, [_fp, C.POINTER(C.c_int32), C.c_int, _fp, C.c_double, C.c_double, _fp, _fp, _fp] + [C.c_int] * 4 +
+                           [_fp, C.c_size_t, _fp]),
     'cg_latent_l1': (C.c_int, [_fp, _fp, C.c_int, _fp, _fp, C.c_float, C.c_int, _fp, C.c_int, C.c_long, _fp, C.c_size_t, _fp]),
     'cg_recon_finalize': (C.c_int, [_fp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int, C.c_int, _fp, _fp, _fp, C.c_size_t,
                                     _fp]),
@@ -628,6 +631,37 @@ class CudaOps:
         ws = self._loss_scratch(G)  # never grows the scratch: a new buffer would drop the accumulator gen_loss_bwd left in it
         self._ck(self.lib.cg_abs_beginning_end_bwd(_p(x_fake), _p(x), _p(sums), float(numel), w, _p(total), _p(pub), _p(d_x), G, B, H, W,
                                                    _p(ws), ws.numel(), self._stream()), 'cg_abs_beginning_end_bwd')
+
+    def council_abs_fwd(self, x_fake, peers, gray, sums):
+        """Pass 1 of council_abs_w: sums[g] = sum |x_fake[g] - x_fake[peers[g]]| over the 3 live lanes (gray: of the channel sums) on
+        this rank.  x_fake [G,B,H,W,4]; peers: G python ints, each another member.  ONE launch."""
+        self._chk(x_fake, sums)
+        G, B, H, W, _ = x_fake.shape
+        assert len(peers) == G and sums.numel() == G
+        ws = self._loss_scratch(G, B, H, W)
+        self._timed_raw('hbm:council_abs_fwd G%d B%d %dx%d' % (G, B, H, W), 4.0 * 2 * x_fake.numel(),
+                        lambda: self._ck(self.lib.cg_council_abs_fwd(_p(x_fake), (C.c_int32 * G)(*peers), int(bool(gray)), _p(sums), G, B, H,
+                                                                     W, _p(ws), ws.numel(), self._stream()), 'cg_council_abs_fwd'))
+
+    def council_abs_bwd(self, x_fake, peers, gray, sums, numel, w, total, pub, d_x):
+        """Pass 2: pub[g] = w * sums[g] / numel (the weighted term), total[g] += pub[g], d_x[g] += w / numel * sign(d) on the 3 live
+        lanes; the peers take no gradient.  numel: of the GLOBAL minibatch.  Must follow gen_loss_bwd of the same direction (the
+        direction totals share its double accumulator).  ONE launch."""
+        self._chk(x_fake, sums, total, pub, d_x)
+        G, B, H, W, _ = x_fake.shape
+        assert tuple(d_x.shape) == tuple(x_fake.shape) and len(peers) == G
+        ws = self._loss_scratch(G)  # never grows the scratch: a new buffer would drop the accumulator gen_loss_bwd left in it
+        self._timed_raw('hbm:council_abs_bwd G%d B%d %dx%d' % (G, B, H, W), 4.0 * 4 * x_fake.numel(),
+                        lambda: self._ck(self.lib.cg_council_abs_bwd(_p(x_fake), (C.c_int32 * G)(*peers), int(bool(gray)), _p(sums),
+                                                                     float(numel), float(w), _p(total), _p(pub), _p(d_x), G, B, H, W,
+                                                                     _p(ws), ws.numel(), self._stream()), 'cg_council_abs_bwd'))
+
+    def add_column(self, dst, k, src):
+        """dst[:, k] += src for dst [n, C] and src [n] (contiguous), one launch"""
+        self._chk(dst, src)
+        n, Cd = dst.shape
+        assert src.numel() == n and 0 <= k < Cd
+        self._ck(self.lib.cg_acc_slice(dst.data_ptr() + 4 * k, _p(src), n, Cd, 1, 1, self._stream()), 'cg_acc_slice')
 
     def latent_l1(self, a, b, sums, coef, da=None, db=None, accumulate=False):
         """recon_criterion(a, b) = mean |a - b| per member (recon_c / recon_s): sums[g] = sum |a - b| of member g on this rank; in the

@@ -43,7 +43,14 @@ What is different underneath (GPU-first, see DESIGN.md):
     decoder, head and MLP gradients go into a scratch added after that generator's own decoder backward, d(content) joins the
     content gradient, and d(style) trains this generator's style encoder on the source image (summed with recon_s's pass when both
     are on).  The reconstruction's mask takes no loss.  With recon_x_w 0 (the shipped configs) nothing of it runs.
-Paths outside the live configuration space of the reference's three configs (recon_x_cyc / vgg / council_abs losses,
+  * council_abs_w (:224-228, 595-619, the council loss without a discriminator; both directions required): while the council gate is
+    open, one peer per member is drawn on the host with ``random.choice`` in member order (the reference's draw; it serves both
+    directions), and two launches per direction compute mean |x_i - x_peer| (or of the channel sums with council_abs_gray_scale) and
+    its gradient, the peer detached; the sums join the scalar all-reduce.  Each direction's term is published in the OTHER
+    direction's council list (``council_loss_ab_s`` holds the b2a term, as :616-619 do).  With council_w 0 there are no council
+    discriminators and dis_council_update returns at once.  With council_abs_w 0 (the shipped configs) nothing of it runs and
+    gen_update draws nothing from ``random``.
+Paths outside the live configuration space of the reference's three configs (recon_x_cyc / vgg losses,
 nsgan/RaHinge, do_my_style, gray-scale D, random D/G pairing) raise NotImplementedError.
 """
 from __future__ import annotations
@@ -233,12 +240,15 @@ class Council_Trainer(nn.Module):
     # ------------------------------------------------------------------------------------------------
     @staticmethod
     def _check_supported(hp):
-        bad = [k for k in ('recon_x_cyc_w', 'vgg_w', 'council_abs_w') if hp.get(k, 0) != 0]
+        bad = [k for k in ('recon_x_cyc_w', 'vgg_w') if hp.get(k, 0) != 0]
         if bad:
             raise NotImplementedError('loss terms %s are not on the accelerated training path' % bad)
         if any(hp.get(k, 0) != 0 for k in ('recon_x_w', 'recon_c_w', 'recon_s_w')) and not (hp['do_a2b'] and hp['do_b2a']):
             raise NotImplementedError('recon_x_w / recon_c_w / recon_s_w decode or re-encode with the other direction\'s generator, so '
                                       'they need do_a2b and do_b2a (with one direction the reference fails with an IndexError)')
+        if hp.get('council_abs_w', 0) != 0 and not (hp['do_a2b'] and hp['do_b2a']):
+            raise NotImplementedError('council_abs_w publishes each direction\'s term with the other direction\'s council loss, so it '
+                                      'needs do_a2b and do_b2a (with one direction the reference fails with an AttributeError)')
         if hp['dis']['gan_type'] != 'lsgan':
             assert 0, "Unsupported GAN type: {}".format(hp['dis']['gan_type'])
         if hp['dis'].get('do_Dis_only_gray') or hp['dis'].get('useRandomGen') or hp['gen'].get('useRandomDis'):
@@ -568,6 +578,11 @@ class Council_Trainer(nn.Module):
                 'at leas one small mask loss should be true, mask_small_use_abs or mask_small_use_square'
         self.do_council_loss = self._gate(hp, for_gen=True)
         council_on = (hp['council_w'] != 0) and self.do_council_loss and N > 1 and self.do_dis_council  # :559,567
+        ca_w = hp['council_abs_w']
+        ca_on = ca_w != 0 and self.do_council_loss and N > 1  # :559,595
+        if ca_on:  # :596-597: one peer per member, in member order, serving both directions
+            peers = [random.choice(list(range(0, i)) + list(range(i + 1, N))) for i in range(N)]
+            ca_gray = bool(hp['council_abs_gray_scale'])
         gan_on = hp['gan_w'] != 0
         center, eps = float(fl['mask_zero_or_one_center']), float(fl['mask_zero_or_one_epsilon'])
         be_w = self._abs_beginning_end_weights(hp, iterations)
@@ -581,12 +596,14 @@ class Council_Trainer(nn.Module):
         # ---- forward of every direction; pass 1 of the loss (all reductions, one launch per direction) -----------
         fw = {}
         nd = len(self._dirs)
-        extra = (nd * N * 2 if be_on else 0) + len(recon) * N
-        if extra:  # the abs_beginning_end sums [|d|, d^2] and the recon sums ride behind the other scalars: still one all-reduce
-            red = ops.empty(nd * N * 6 + extra)
+        extra = (nd * N * 2 if be_on else 0) + (nd * N if ca_on else 0) + len(recon) * N
+        if extra:  # the abs_beginning_end sums [|d|, d^2], the council abs sums and the recon sums ride behind the other scalars:
+            red = ops.empty(nd * N * 6 + extra)  # still one all-reduce
             scal, off = red[:nd * N * 6].view(nd, N, 6), nd * N * 6
             if be_on:
                 be_sums, off = red[off:off + nd * N * 2].view(nd, N, 2), off + nd * N * 2
+            if ca_on:
+                ca_sums, off = red[off:off + nd * N].view(nd, N), off + nd * N
             if recon:
                 rc_sums = red[off:].view(len(recon), N)
         else:
@@ -616,6 +633,8 @@ class Council_Trainer(nn.Module):
                                             float(hp['gan_w']) / self.world, scal[di])
             if be_on:
                 ops.abs_beginning_end_fwd(x_fake, src, be_sums[di])
+            if ca_on:
+                ops.council_abs_fwd(x_fake, peers, ca_gray, ca_sums[di])
             if recon:
                 rec['c'], rec['src'] = c, src
             fw[d] = rec
@@ -633,6 +652,8 @@ class Council_Trainer(nn.Module):
         if be_on:
             be_pub = ops.empty(nd, N)
             be_weights = [float(w) for w in be_w] + [0.0] * (N - len(be_w))  # 0: this member's gate is closed
+        if ca_on:
+            ca_pub = ops.empty(nd, N)
         matching = bool(self.do_w_loss_matching)
         data_parallel = self.world > 1
         recon_x_on = hp['recon_x_w'] != 0
@@ -677,6 +698,9 @@ class Council_Trainer(nn.Module):
             if be_on:  # after gen_loss_bwd of this direction: the totals share its accumulator
                 ops.abs_beginning_end_bwd(rec['x_fake'], self._src(d, img_a, img_b), be_sums[di], hpd['numel'], be_weights, total,
                                           be_pub[di], d_x)
+            if ca_on:  # likewise after gen_loss_bwd of this direction
+                numel = rec['B'] * self.world * rec['H'] * rec['W'] * (1 if ca_gray else 3)
+                ops.council_abs_bwd(rec['x_fake'], peers, ca_gray, ca_sums[di], numel, float(ca_w), total, ca_pub[di], d_x)
             gen.backward(d_x, d_mask, rec['enc'], rec['dec'],
                          on_decoder_done=(lambda g=gen: decoder_done(g)) if recon_x_on or data_parallel else None,
                          d_content=rec.get('d_c'))
@@ -687,6 +711,9 @@ class Council_Trainer(nn.Module):
         if recon:  # after every gen_loss_bwd / abs_beginning_end_bwd of this update: the member totals share their accumulator
             rc_pub = ops.empty(len(recon), N)
             ops.recon_finalize(rc_sums, recon_numel, [float(w) for _, _, w in recon], total, rc_pub)
+        if ca_on:  # :616-619: each direction's published council loss takes the OTHER direction's abs term (both directions are on)
+            for di in range(nd):
+                ops.add_column(pub[di], 5, ca_pub[nd - 1 - di])
         self._adam('gen', defer=True)  # joined at the start of the next update (or by save / state_dict / sample)
         self._enc_cache.clear()
 
@@ -703,7 +730,7 @@ class Council_Trainer(nn.Module):
                 setattr(self, 'loss_gen_mask_zero_one_%s_s' % ab, col(2, focus_on and hp['mask_zero_or_one_w'] != 0))
                 setattr(self, 'loss_gen_mask_total_%s_s' % ab, col(3) if focus_on and hp['mask_total_w'] != 0 else [0] * N)
                 setattr(self, 'loss_gen_mask_TV_%s_s' % ab, col(4) if focus_on and hp['mask_tv_w'] != 0 else [0] * N)
-                setattr(self, 'council_loss_%s_s' % ab, col(5) if council_on else [0] * N)
+                setattr(self, 'council_loss_%s_s' % ab, col(5) if council_on or ca_on else [0] * N)
                 if council_on and matching:
                     setattr(self, 'w_match_%s_conf' % d, pub[di, N - 1, 6])  # the reference keeps the last member's ratio (:583)
             else:

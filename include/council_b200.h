@@ -166,8 +166,8 @@ int cg_focus_fwd(const float* mask, float* sums, int G, int B, int H, int W, flo
 int cg_focus_bwd(const float* mask, const float* coef, float* dmask, int G, int B, int H, int W,
                  float center, float eps, void* stream);
 
-/* ---- fused losses (one launch per discriminator update and direction; two per gen_update and direction, two more with
- *      abs_beginning_end on) --------------------------------------------------------------------------------------------
+/* ---- fused losses (one launch per discriminator update and direction; two per gen_update and direction, two more each with
+ *      abs_beginning_end or council_abs_w on) -------------------------------------------------------------------------
  * These replace the four calls above on the training path: the loss of EVERY discriminator scale, the focus terms, the
  * loss-history matching and all their gradients, with no host round trip (trainer_council.py:518-524,576-586 run on the
  * device).  `ws`: >= cg_loss_workspace_bytes() bytes, ZERO-INITIALISED once by the caller, not shared between streams;
@@ -231,6 +231,18 @@ int cg_abs_beginning_end_fwd(const float* x_fake, const float* x, float* sums, i
 int cg_abs_beginning_end_bwd(const float* x_fake, const float* x, const float* sums, double numel, const double* host_weight,
                              float* total, float* pub, float* d_x, int G, int B, int H, int W, void* ws, size_t ws_bytes,
                              void* stream);
+/* council abs loss, council_abs_w (trainer_council.py:224-228, 595-619): member g's translation x_fake[g] against the detached
+ * translation of its peer x_fake[host_peer[g]], x_fake[G][B][H][W][4]; colour: |d| on the 3 live lanes, gray: |sum_c x_g - sum_c x_p|
+ * per pixel.  host_peer[G] (host memory, passed by value) must name another member: G <= CG_LOSS_MAX_G, 0 <= peer < G, peer != g.
+ * pass 1: sums[g] = the sum of those over member g on this rank (float partials per block, added in double; fixed order). */
+int cg_council_abs_fwd(const float* x_fake, const int32_t* host_peer, int gray, float* sums, int G, int B, int H, int W, void* ws,
+                       size_t ws_bytes, void* stream);
+/* pass 2 (sums summed over ranks; numel = (gray ? 1 : 3)*H*W*B of the GLOBAL minibatch): pub[g] = w * sums[g] / numel (the weighted
+ * term); total[g] += pub[g] through the double accumulator cg_gen_loss_bwd keeps in the same workspace, so it must follow the
+ * cg_gen_loss_bwd call of the same direction on the same workspace and stream; d_x[g] += w / numel * sign(d) on lanes 0..2 (gray: the
+ * sign of the channel-sum difference on all three; sign(0) = 0).  Lane 3 keeps its value; the peer takes no gradient. */
+int cg_council_abs_bwd(const float* x_fake, const int32_t* host_peer, int gray, const float* sums, double numel, double w, float* total,
+                       float* pub, float* d_x, int G, int B, int H, int W, void* ws, size_t ws_bytes, void* stream);
 /* latent reconstruction, recon_c_w / recon_s_w (trainer_council.py:359-369, 460-469): recon_criterion(a, b) = mean |a - b| of a
  * re-encoded code a[G][n] against its target b ([G][n], or [n] shared by all members when b_shared).
  * sums[g] = sum |a - b| over member g on this rank (float partials per block, added in double; fixed order), and in the same pass
