@@ -192,6 +192,64 @@ __global__ void gather_images_kernel(const float* __restrict__ pool0, int n0, co
     }
 }
 
+// do_Dis_only_gray (trainer_council.py:736-737, 761, 765, 504, 510): torch.sum(x, 1) / input_dim on every live lane -- the sum in
+// channel order, then a true division -- and 0 on lane 3
+__global__ void gather_images_gray_kernel(const float* __restrict__ pool0, int n0, const float* __restrict__ pool1,
+                                          const int32_t* __restrict__ idx, float* __restrict__ y, long total, int HW) {
+    pdl_trigger();
+    pdl_wait();
+    long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    int pix = (int)(i % HW);
+    int slot = __ldg(idx + i / HW);
+    float4 v = slot < n0 ? f4(pool0 + ((long)slot * HW + pix) * 4) : f4(pool1 + ((long)(slot - n0) * HW + pix) * 4);
+    float g = __fdiv_rn(v.x + v.y + v.z, 3.f);
+    reinterpret_cast<float4*>(y)[i] = make_float4(g, g, g, 0.f);
+}
+
+// autograd of the conversion above: d x_c = g0/3 + g1/3 + g2/3 on every live lane (the division's gradient, then the repeat's sum)
+__global__ void gray_fold_kernel(float* __restrict__ d, long npix) {
+    pdl_trigger();
+    pdl_wait();
+    long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= npix) return;
+    float4 v = reinterpret_cast<const float4*>(d)[i];
+    float g = __fdiv_rn(v.x, 3.f) + __fdiv_rn(v.y, 3.f) + __fdiv_rn(v.z, 3.f);
+    reinterpret_cast<float4*>(d)[i] = make_float4(g, g, g, v.w);
+}
+
+// useRandomDis (trainer_council.py:499-501): dst[g] = src[map[g]] in every member-major segment [G][n] of a parameter bank.  Blocks
+// are dealt to the segments in proportion to their size (blk0[s] = first block of segment s), so no block idles.
+constexpr int GM_THREADS = 256, GM_UNROLL = 4;
+struct MemberGather {
+    int map[CG_LOSS_MAX_G];
+    int G, nseg;
+    long off[CG_GATHER_MAX_SEG], n[CG_GATHER_MAX_SEG];  // floats: segment start, per-member length
+    int blk0[CG_GATHER_MAX_SEG + 1];
+};
+__global__ void __launch_bounds__(GM_THREADS) gather_members_kernel(const float* __restrict__ src, float* __restrict__ dst,
+                                                                    const MemberGather mg) {
+    pdl_trigger();
+    pdl_wait();
+    int s = 0;
+    while (s + 1 < mg.nseg && (int)blockIdx.x >= mg.blk0[s + 1]) s++;
+    const long n = mg.n[s], off = mg.off[s];
+    const bool vec = (n & 3) == 0;  // segment starts are 64-float aligned
+    const long per = vec ? n / 4 : n, total = per * mg.G;
+    const long base = (long)(blockIdx.x - mg.blk0[s]) * GM_THREADS * GM_UNROLL + threadIdx.x;
+#pragma unroll
+    for (int u = 0; u < GM_UNROLL; u++) {
+        const long i = base + (long)u * GM_THREADS;
+        if (i >= total) break;
+        const long g = i / per, k = i - g * per;
+        const long from = (long)mg.map[g] * per + k;
+        if (vec)
+            reinterpret_cast<float4*>(dst + off)[i] = __ldg(reinterpret_cast<const float4*>(src + off) + from);
+        else
+            dst[off + i] = __ldg(src + off + from);
+    }
+}
+
 __global__ void nchw_to_nhwc_kernel(const float* __restrict__ x, float* __restrict__ y, long total, int C, int HW, int Cp) {
     pdl_trigger();
     pdl_wait();
@@ -389,6 +447,49 @@ extern "C" int cg_gather_images(const float* pool0, int n0, const float* pool1, 
     long total = (long)G * Bt * HW;
     launch_k(gather_images_kernel, cdiv(total, 256), 256, 0, ST, pool0, n0, pool1, idx, x_in, y, total, Bt, B, HW);
     return check_launch("gather_images");
+}
+extern "C" int cg_gather_images_gray(const float* pool0, int n0, const float* pool1, const int32_t* idx, const float* x_in, float* y,
+                                     int G, int Bt, int B, int HW, void* stream) {
+    CG_REQUIRE(!x_in, "gather_images_gray: x_in must be NULL (the council discriminators see colour)");
+    CG_REQUIRE(pool0 && idx && y && G >= 1 && Bt >= 1 && B >= 1 && HW >= 1, "gather_images_gray: G=%d Bt=%d HW=%d out of range", G,
+               Bt, HW);
+    long total = (long)G * Bt * HW;
+    launch_k(gather_images_gray_kernel, cdiv(total, 256), 256, 0, ST, pool0, n0, pool1, idx, y, total, HW);
+    return check_launch("gather_images_gray");
+}
+extern "C" int cg_gray_fold(float* d_x, long npix, void* stream) {
+    CG_REQUIRE(d_x && npix >= 1, "gray_fold: npix=%ld out of range", npix);
+    launch_k(gray_fold_kernel, cdiv(npix, 256), 256, 0, ST, d_x, npix);
+    return check_launch("gray_fold");
+}
+extern "C" int cg_gather_members(const float* src, float* dst, const int64_t* host_off, const int64_t* host_n, int nseg,
+                                 const int32_t* host_map, int G, void* stream) {
+    CG_REQUIRE(src && dst && host_off && host_n && host_map, "gather_members: NULL argument");
+    CG_REQUIRE(G >= 1 && G <= CG_LOSS_MAX_G, "gather_members: G=%d out of range (1..%d)", G, CG_LOSS_MAX_G);
+    CG_REQUIRE(nseg >= 1 && nseg <= CG_GATHER_MAX_SEG, "gather_members: nseg=%d out of range (1..%d)", nseg, CG_GATHER_MAX_SEG);
+    MemberGather mg;
+    mg.G = G;
+    mg.nseg = nseg;
+    for (int g = 0; g < G; g++) {
+        CG_REQUIRE(host_map[g] >= 0 && host_map[g] < G, "gather_members: map[%d] = %d is not a member", g, host_map[g]);
+        mg.map[g] = host_map[g];
+    }
+    long blocks = 0;
+    for (int s = 0; s < nseg; s++) {
+        CG_REQUIRE(host_off[s] >= 0 && host_n[s] >= 1, "gather_members: segment %d (off %lld, n %lld) out of range", s,
+                   (long long)host_off[s], (long long)host_n[s]);
+        CG_REQUIRE(host_off[s] % 4 == 0, "gather_members: segment %d starts at %lld, not a multiple of 4 floats", s,
+                   (long long)host_off[s]);
+        mg.off[s] = host_off[s];
+        mg.n[s] = host_n[s];
+        mg.blk0[s] = (int)blocks;
+        const long per = host_n[s] % 4 == 0 ? host_n[s] / 4 : host_n[s];
+        blocks += cdiv(per * G, (long)GM_THREADS * GM_UNROLL);
+        CG_REQUIRE(blocks < (1L << 31), "gather_members: too many blocks");
+    }
+    mg.blk0[nseg] = (int)blocks;
+    launch_k(gather_members_kernel, (int)blocks, GM_THREADS, 0, ST, src, dst, mg);
+    return check_launch("gather_members");
 }
 extern "C" int cg_nchw_to_nhwc(const float* x, float* y, int N, int C, int HW, int Cp, void* stream) {
     long total = (long)N * HW;

@@ -72,6 +72,10 @@ class ParamBank:
     def p(self, name):
         return self._view(self.data, name)
 
+    def member_segments(self):
+        """[(offset, floats per member)] of every entry: the member-major segments of ops.gather_members"""
+        return [(off, n // self.G) for off, _, n in self.table.values()]
+
     def g(self, name):
         return self._view(self.grad, name)
 
@@ -670,12 +674,17 @@ class CouncilDis(_StackedNet):
     def _banks(self):
         return (self.bank,)
 
+    def bank_like(self):
+        """a parameter bank with self.bank's layout, data only (zero-initialised)"""
+        return ParamBank(self.ops, self.G, [e for s in self.specs for e in s.entries()], trainable=False)
+
     def reference_key_order(self):
         return [k for s in self.specs for k in (s.wname, s.bname)]
 
-    def forward(self, x, saved=None):
-        """x [G,Bt,H,W,4|8] -> list over scales of patch outputs [G,Bt,h,w,1]."""
-        ops, bank = self.ops, self.bank
+    def forward(self, x, saved=None, bank=None):
+        """x [G,Bt,H,W,4|8] -> list over scales of patch outputs [G,Bt,h,w,1].  bank: parameters laid out like self.bank (None:
+        self.bank), e.g. members drawn from it by ops.gather_members."""
+        ops, bank = self.ops, self.bank if bank is None else bank
         outs = []
         for sc, (layers, tail) in enumerate(self.scales):
             h = x
@@ -693,10 +702,11 @@ class CouncilDis(_StackedNet):
                 x = ops.avgpool_fwd(x)
         return outs
 
-    def backward(self, d_outs, saved, want_wgrad, want_dx):
+    def backward(self, d_outs, saved, want_wgrad, want_dx, bank=None):
         """d_outs: per-scale d(loss)/d(out).  want_wgrad: fill bank.grad (dis/dis_council update).
-        want_dx: return d(loss)/d(x) [G,Bt,H,W,lanes of x] accumulated over scales (gen_update)."""
-        ops, bank = self.ops, self.bank
+        want_dx: return d(loss)/d(x) [G,Bt,H,W,lanes of x] accumulated over scales (gen_update).  bank: the parameters forward ran
+        with (None: self.bank)."""
+        ops, bank = self.ops, self.bank if bank is None else bank
         dx_scales = []
         for sc, (layers, tail) in enumerate(self.scales):
             acts = saved[sc]

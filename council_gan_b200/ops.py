@@ -72,6 +72,9 @@ _SIGS = {
     'cg_avgpool_bwd': (C.c_int, [_fp, _fp] + [C.c_int] * 7 + [_fp]),
     'cg_acc_slice': (C.c_int, [_fp, _fp, C.c_long, C.c_int, C.c_int, C.c_int, _fp]),
     'cg_gather_images': (C.c_int, [_fp, C.c_int, _fp, _fp, _fp, _fp, C.c_int, C.c_int, C.c_int, C.c_int, _fp]),
+    'cg_gather_images_gray': (C.c_int, [_fp, C.c_int, _fp, _fp, _fp, _fp, C.c_int, C.c_int, C.c_int, C.c_int, _fp]),
+    'cg_gray_fold': (C.c_int, [_fp, C.c_long, _fp]),
+    'cg_gather_members': (C.c_int, [_fp, _fp, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int, C.POINTER(C.c_int32), C.c_int, _fp]),
     'cg_nchw_to_nhwc': (C.c_int, [_fp, _fp, C.c_int, C.c_int, C.c_int, C.c_int, _fp]),
     'cg_nhwc_to_nchw': (C.c_int, [_fp, _fp, C.c_int, C.c_int, C.c_int, C.c_int, _fp]),
     'cg_lsgan_fwd': (C.c_int, [_fp, _fp, _fp, _fp, _fp, C.c_int, C.c_int, C.c_int, C.c_int, _fp]),
@@ -449,6 +452,41 @@ class CudaOps:
         self._ck(self.lib.cg_gather_images(_p(pools[0]), S0, _p(p1), idx.data_ptr(), _p(x_in), _p(y), G, Bt, B, H * W,
                                            self._stream()), 'cg_gather_images')
         return y
+
+    def gather_images_gray(self, pools, idx, G, Bt):
+        """gather_images without x_in, each slot converted to gray scale (do_Dis_only_gray): {m, m, m, 0}, m = (x0 + x1 + x2) / 3
+        -> [G,Bt,H,W,4]"""
+        if torch.is_tensor(pools):
+            pools = (pools,)
+        self._chk(*pools)
+        assert idx.dtype == torch.int32 and idx.is_cuda and idx.is_contiguous() and idx.numel() == G * Bt
+        S0, H, W, _ = pools[0].shape
+        p1 = pools[1] if len(pools) > 1 else None
+        y = self.empty(G, Bt, H, W, 4)
+        self._timed_raw('hbm:gather_images_gray G%d Bt%d %dx%d' % (G, Bt, H, W), 4.0 * 2 * y.numel(),
+                        lambda: self._ck(self.lib.cg_gather_images_gray(_p(pools[0]), S0, _p(p1), idx.data_ptr(), None, _p(y), G, Bt, 1,
+                                                                        H * W, self._stream()), 'cg_gather_images_gray'))
+        return y
+
+    def gray_fold(self, d_x):
+        """in place on a data gradient [..., 4] w.r.t. a gray_images input: lanes 0..2 = g0/3 + g1/3 + g2/3, lane 3 kept"""
+        self._chk(d_x)
+        assert d_x.shape[-1] == 4
+        self._timed_raw('hbm:gray_fold n%d' % d_x.numel(), 4.0 * 2 * d_x.numel(),
+                        lambda: self._ck(self.lib.cg_gray_fold(_p(d_x), d_x.numel() // 4, self._stream()), 'cg_gray_fold'))
+
+    def gather_members(self, src, dst, segments, member_map):
+        """dst[g] = src[member_map[g]] in every member-major segment (offset, floats per member) of two flat buffers laid out
+        alike (the data of two ParamBanks with one table).  member_map: G python ints.  ONE launch."""
+        self._chk(src, dst)
+        G = len(member_map)
+        assert src.numel() == dst.numel() and len(segments) >= 1
+        nseg = len(segments)
+        off = (C.c_int64 * nseg)(*[o for o, _ in segments])
+        n = (C.c_int64 * nseg)(*[k for _, k in segments])
+        self._timed_raw('hbm:gather_members G%d n%d' % (G, src.numel()), 4.0 * 2 * G * sum(k for _, k in segments),
+                        lambda: self._ck(self.lib.cg_gather_members(_p(src), _p(dst), off, n, nseg, (C.c_int32 * G)(*member_map), G,
+                                                                    self._stream()), 'cg_gather_members'))
 
     # -- host -> device staging -------------------------------------------------------------------
     def stage(self, arrays):

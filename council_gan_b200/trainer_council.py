@@ -50,8 +50,16 @@ What is different underneath (GPU-first, see DESIGN.md):
     direction's council list (``council_loss_ab_s`` holds the b2a term, as :616-619 do).  With council_w 0 there are no council
     discriminators and dis_council_update returns at once.  With council_abs_w 0 (the shipped configs) nothing of it runs and
     gen_update draws nothing from ``random``.
+  * do_Dis_only_gray / useRandomGen / useRandomDis (:499-510, 736-765, the discriminator-side switches): with gray scale D sees
+    sum_c x / 3 on every live lane -- dis_update gathers its minibatch through a converting gather, gen_update converts the
+    translations and folds D's data gradient back to colour before the council discriminator's colour gradient joins it.  With
+    useRandomGen dis_update draws one generator per member from numpy (np.random.randint, member order, both directions) and D_g
+    trains on that generator's slot of the stacked translations; the table goes up with the style noise.  With useRandomDis (and
+    gan_w != 0) gen_update draws one discriminator per member and runs D on a scratch bank whose member g holds discriminator
+    dis_map[g]'s parameters (one gather launch per direction).  Under data parallelism every rank must seed numpy identically.  With
+    all three off (the shipped configs) nothing of it runs and neither update draws from numpy.
 Paths outside the live configuration space of the reference's three configs (recon_x_cyc / vgg losses,
-nsgan/RaHinge, do_my_style, gray-scale D, random D/G pairing) raise NotImplementedError.
+nsgan/RaHinge, do_my_style, do_w_loss_matching_focus) raise NotImplementedError.
 """
 from __future__ import annotations
 
@@ -203,6 +211,7 @@ class Council_Trainer(nn.Module):
         self._img_cache = {}
         self._enc_cache = {}
         self._idx_cache = {}
+        self._dis_pick = {}  # direction -> scratch bank of the discriminators gen_update draws with useRandomDis
         self.img_cache_misses = 0  # image batches uploaded / converted (bench.py checks its e2e leg really copies)
         object.__setattr__(self, '_pending', {})  # family -> [(net, bucket, async work)] awaiting all-reduce completion + Adam
         self.hyperparameters = hp
@@ -251,8 +260,6 @@ class Council_Trainer(nn.Module):
                                       'needs do_a2b and do_b2a (with one direction the reference fails with an AttributeError)')
         if hp['dis']['gan_type'] != 'lsgan':
             assert 0, "Unsupported GAN type: {}".format(hp['dis']['gan_type'])
-        if hp['dis'].get('do_Dis_only_gray') or hp['dis'].get('useRandomGen') or hp['gen'].get('useRandomDis'):
-            raise NotImplementedError('gray-scale D / random D-G pairing are not on the accelerated path')
         if hp['focus_loss'].get('do_w_loss_matching_focus'):
             raise NotImplementedError('do_w_loss_matching_focus is not on the accelerated path')
         if not (hp['do_a2b'] or hp['do_b2a']):
@@ -435,13 +442,24 @@ class Council_Trainer(nn.Module):
         self._check_supported(hp)
         self._flush()
         ops, N = self.ops, self.council_size
+        gray = bool(hp['dis'].get('do_Dis_only_gray'))
+        # useRandomGen (:748-750): D_g trains on the translation of generator gen_map[g], one draw per member serving both directions
+        gen_map = [int(np.random.randint(N)) for _ in range(N)] if hp['dis'].get('useRandomGen') else None
         img_a, img_b = self._img(x_a), self._img(x_b)
         noise = []
         if self.do_a2b_conf:  # :740-745
             noise.append(('a2b', self._noise(self._bsz(x_b))))
         if self.do_b2a_conf:
             noise.append(('b2a', self._noise(self._bsz(x_a))))
-        s = dict(zip((k for k, _ in noise), ops.stage([v for _, v in noise])))
+        tables = []
+        if gen_map is not None:  # slot tables [translation of gen_map[g] ; real], in the same pinned copy as the noise
+            for d in self._dirs:
+                B = self._bsz(self._src(d, x_a, x_b))
+                tables.append(torch.tensor([[gen_map[g] * B + b for b in range(B)] + [N * B + b for b in range(B)] for g in range(N)],
+                                           dtype=torch.int32))
+        dev = ops.stage([v for _, v in noise] + tables)
+        s = dict(zip((k for k, _ in noise), dev[:len(noise)]))
+        random_idx = dict(zip(self._dirs, dev[len(noise):]))
         total = ops.empty(N)
         inv_world = 1.0 / self.world
         for di, d in enumerate(self._dirs):
@@ -451,9 +469,13 @@ class Council_Trainer(nn.Module):
             c, _ = self._encode(d, src, save=True)
             x_fake, _ = gen.decode(c, s[d], src)
             # D minibatch per member: [own fake ; real]   (calc_dis_loss networks.py:56-64); slots >= N*B read the real batch
-            idx = self._idx(('dis', N, B), lambda: [[g * B + b for b in range(B)] + [N * B + b for b in range(B)]
-                                                    for g in range(N)])
-            xin = ops.gather_images((x_fake.view(N * B, H, W, IMG_C), real[0]), idx, None, N, 2 * B)
+            idx = random_idx.get(d)
+            if idx is None:
+                idx = self._idx(('dis', N, B), lambda: [[g * B + b for b in range(B)] + [N * B + b for b in range(B)]
+                                                        for g in range(N)])
+            pools = (x_fake.view(N * B, H, W, IMG_C), real[0])
+            # do_Dis_only_gray (:736-737, 761, 765): D sees the translation and the real batch in gray scale
+            xin = ops.gather_images_gray(pools, idx, N, 2 * B) if gray else ops.gather_images(pools, idx, None, N, 2 * B)
             saved = []
             outs = dis.forward(xin, saved)
             wdir = float(hp['gan_w']) if d == 'a2b' else 1.0  # :775 vs :777 (no gan_w on the b2a branch)
@@ -584,6 +606,10 @@ class Council_Trainer(nn.Module):
             peers = [random.choice(list(range(0, i)) + list(range(i + 1, N))) for i in range(N)]
             ca_gray = bool(hp['council_abs_gray_scale'])
         gan_on = hp['gan_w'] != 0
+        # useRandomDis (:499-501, only with gan_w != 0): member g's adversarial loss comes from discriminator dis_map[g], drawn in member
+        # order from numpy; its loss history and w_match stay member g's
+        dis_map = [int(np.random.randint(N)) for _ in range(N)] if gan_on and hp['gen'].get('useRandomDis') else None
+        dis_gray = bool(hp['dis'].get('do_Dis_only_gray'))
         center, eps = float(fl['mask_zero_or_one_center']), float(fl['mask_zero_or_one_epsilon'])
         be_w = self._abs_beginning_end_weights(hp, iterations)
         be_on = bool(be_w)
@@ -620,8 +646,13 @@ class Council_Trainer(nn.Module):
             if gan_on:  # calc_gen_loss networks.py:84-90
                 if di == 0:
                     self._finish('dis')
+                rec['dis_bank'] = self._dis_members(d, dis_map) if dis_map is not None else None
+                x_dis = x_fake
+                if dis_gray:  # :504, 510: D sees the gray translation; the gradient flows back through the conversion
+                    idx = self._idx(('id', N, B), lambda: [[g * B + b for b in range(B)] for g in range(N)])
+                    x_dis = ops.gather_images_gray(x_fake.view(N * B, H, W, IMG_C), idx, N, B)
                 rec['dis_saved'] = []
-                rec['dis_outs'] = self._nets['dis_' + d].forward(x_fake, rec['dis_saved'])
+                rec['dis_outs'] = self._nets['dis_' + d].forward(x_dis, rec['dis_saved'], bank=rec['dis_bank'])
             if council_on:  # MsImageDisCouncil.calc_gen_loss networks.py:188-194
                 if di == 0:
                     self._finish('dis_council')
@@ -682,7 +713,9 @@ class Council_Trainer(nn.Module):
                 ring['head_council'] = (ring['head_council'] + 1) % R
             d_x = None
             if gan_on:
-                d_x = self._nets['dis_' + d].backward(rec['d_adv'], rec['dis_saved'], want_wgrad=False, want_dx=True)
+                d_x = self._nets['dis_' + d].backward(rec['d_adv'], rec['dis_saved'], want_wgrad=False, want_dx=True, bank=rec['dis_bank'])
+                if dis_gray:  # before the council discriminator's colour gradient joins d_x
+                    ops.gray_fold(d_x)
             if council_on:
                 d_x8 = self._nets['dis_council_' + d].backward(d_cl, rec['disc_saved'], want_wgrad=False, want_dx=True)
                 if d_x is None:
@@ -749,6 +782,16 @@ class Council_Trainer(nn.Module):
             for k, (kind, dom, _) in enumerate(recon):
                 setattr(self, 'loss_gen_recon_%s_%s_s' % (kind, dom), [rc_pub[k, i] for i in range(N)])
         self._last_fw = {d: {'x_fake': fw[d]['x_fake'], 'mask': fw[d]['mask']} for d in self._dirs}
+
+    def _dis_members(self, d, dis_map):
+        """The discriminators of direction d with member g's parameters copied from member dis_map[g] (useRandomDis), in a scratch bank
+        allocated once per direction: its address stays the same for the tensor-map cache, which is keyed by pointer."""
+        dis = self._nets['dis_' + d]
+        bank = self._dis_pick.get(d)
+        if bank is None:
+            bank = self._dis_pick[d] = dis.bank_like()
+        self.ops.gather_members(dis.bank.data, bank.data, dis.bank.member_segments(), dis_map)
+        return bank
 
     def _recon_forward(self, fw, s, recon, sums):
         """The reconstruction passes, keeping activations for the backward, and their terms: sums[k] = this rank's sum |recon - target|

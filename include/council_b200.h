@@ -146,6 +146,21 @@ int cg_acc_slice(float* dst, const float* src, long npix, int Cd, int Cs, int nc
  * torch.cat((x, x_input), 1) (networks.py:152). */
 int cg_gather_images(const float* pool0, int n0, const float* pool1, const int32_t* idx, const float* x_in, float* y,
                      int G, int Bt, int B, int HW, void* stream);
+/* do_Dis_only_gray (trainer_council.py:736-737, 761, 765, 504, 510): the slots of cg_gather_images (same arguments; x_in must be
+ * NULL) converted to gray scale, y[g][n] = {m, m, m, 0} with m = (x0 + x1 + x2) / 3 (summed in that order, then a true division):
+ * torch.sum(x, 1).unsqueeze(1).repeat(1, input_dim, 1, 1) / input_dim with input_dim = 3. */
+int cg_gather_images_gray(const float* pool0, int n0, const float* pool1, const int32_t* idx, const float* x_in, float* y,
+                          int G, int Bt, int B, int HW, void* stream);
+/* the data gradient through that conversion, in place on d_x[npix][4]: lanes 0..2 = g0/3 + g1/3 + g2/3 (autograd's order);
+ * lane 3 keeps its value */
+int cg_gray_fold(float* d_x, long npix, void* stream);
+/* useRandomDis (trainer_council.py:499-501): a parameter bank with members drawn from another, dst[g] = src[host_map[g]] in each
+ * member-major segment s (floats [host_off[s], host_off[s] + G*host_n[s]) of both buffers, host_off[s] % 4 == 0).  host_map[G]
+ * (host memory, passed by value) may repeat members and map a member to itself: G <= CG_LOSS_MAX_G, 0 <= host_map[g] < G,
+ * nseg <= CG_GATHER_MAX_SEG.  Floats outside the segments are not written. */
+#define CG_GATHER_MAX_SEG 64
+int cg_gather_members(const float* src, float* dst, const int64_t* host_off, const int64_t* host_n, int nseg,
+                      const int32_t* host_map, int G, void* stream);
 /* NCHW [N][C][HW] <-> channels-last [N][HW][Cp] (Cp >= C, pad lanes zeroed) */
 int cg_nchw_to_nhwc(const float* x, float* y, int N, int C, int HW, int Cp, void* stream);
 int cg_nhwc_to_nchw(const float* x, float* y, int N, int C, int HW, int Cp, void* stream);
