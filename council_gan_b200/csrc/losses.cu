@@ -14,6 +14,7 @@
 //   recon_x (recon_criterion of the within-domain decode)   trainer_council.py:339-345, 455-459
 //   council_abs_w (council_basic_criterion_*)               trainer_council.py:224-228, 595-619  (2 more launches per direction
 //                                                           while the council gate is open)
+//   vgg_w (compute_vgg_loss on relu5_3)                     trainer_council.py:531-538, 636-641  (1 launch per update)
 #include "common.cuh"
 #include "mask_head.cuh"
 
@@ -614,6 +615,76 @@ __global__ void __launch_bounds__(256) recon_head_bwd_kernel(const float* __rest
     store12(dh_pre + i * 12, out);
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// gen_update, perceptual loss (vgg_w, trainer_council.py:531-538, 636-641): mean((IN(f_img) - IN(f_tgt))^2) of relu5_3 features,
+// IN = nn.InstanceNorm2d(512, affine=False) (:121), and its gradient w.r.t. conv5_3's pre-activation
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int VL_CH = 32, VL_PY = 8;  // channels x pixel lanes of a 256-thread block
+
+// block (r, chunk) owns channels [32 chunk, 32 chunk + 32) of image row r and pairs it with target row t(r) = (r / per_dir) * B + r % B.
+// Pass 1 over the pixels: z = (f - mean) * rstd of both, d = z_img - z_tgt; the float partial sum d^2 of the block, and per channel
+// mean(g) and mean(g z_img) of g = 2 coef d.  Pass 2: d_pre = rstd (g - mean(g) - z_img mean(g z_img)) (the instance-norm backward,
+// statistics included) times relu5_3's mask f > 0.  The last block adds the partials of each term k (rows [k B, k B + B), the
+// blocks of a row in chunk order) in double: sums[k].
+__global__ void __launch_bounds__(256) vgg_loss_kernel(const float* __restrict__ fi, const float* __restrict__ mi, const float* __restrict__ ri,
+                                                       const float* __restrict__ ft, const float* __restrict__ mt, const float* __restrict__ rt,
+                                                       float coef, float* __restrict__ d_pre, float* __restrict__ sums,
+                                                       float* __restrict__ part, unsigned int* __restrict__ counter, int B, int per_dir,
+                                                       int HW, int C, int nterm) {
+    pdl_trigger();
+    pdl_wait();
+    __shared__ float sm[32];
+    __shared__ float red[2][VL_PY][VL_CH];
+    const int nchunk = C / VL_CH;
+    const int r = blockIdx.x / nchunk, chunk = blockIdx.x - r * nchunk;
+    const int tr = (r / per_dir) * B + r % B;
+    const int lane = threadIdx.x & 31, py = threadIdx.x >> 5;
+    const int c = chunk * VL_CH + lane;
+    const float m_i = __ldg(mi + (long)r * C + c), r_i = __ldg(ri + (long)r * C + c);
+    const float m_t = __ldg(mt + (long)tr * C + c), r_t = __ldg(rt + (long)tr * C + c);
+    const float* fr = fi + (long)r * HW * C + c;
+    const float* ftr = ft + (long)tr * HW * C + c;
+    const float two_coef = 2.f * coef;
+    float v[1] = {0.f};
+    float sg = 0.f, sgz = 0.f;
+    for (int p = py; p < HW; p += VL_PY) {
+        const float zi = (__ldg(fr + (long)p * C) - m_i) * r_i;
+        const float d = zi - (__ldg(ftr + (long)p * C) - m_t) * r_t;
+        v[0] += d * d;
+        const float g = two_coef * d;
+        sg += g;
+        sgz += g * zi;
+    }
+    red[0][py][lane] = sg;
+    red[1][py][lane] = sgz;
+    block_sum<1>(v, sm);  // its barriers also publish red
+    float mg = 0.f, mgz = 0.f;
+#pragma unroll
+    for (int k = 0; k < VL_PY; k++) {
+        mg += red[0][k][lane];
+        mgz += red[1][k][lane];
+    }
+    mg /= (float)HW;
+    mgz /= (float)HW;
+    float* dr = d_pre + (long)r * HW * C + c;
+    for (int p = py; p < HW; p += VL_PY) {
+        const float f = __ldg(fr + (long)p * C);
+        const float zi = (f - m_i) * r_i;
+        const float g = two_coef * (zi - (__ldg(ftr + (long)p * C) - m_t) * r_t);
+        dr[(long)p * C] = f > 0.f ? r_i * (g - mg - zi * mgz) : 0.f;
+    }
+    if (threadIdx.x == 0) part[blockIdx.x] = v[0];
+    if (!last_block_done(counter, gridDim.x)) return;
+    const int t = threadIdx.x;
+    if (t < nterm) {
+        const volatile float* vp = part + (long)t * B * nchunk;
+        double s = 0.0;
+        for (int k = 0; k < B * nchunk; k++) s += (double)vp[k];
+        sums[t] = (float)s;
+    }
+    if (t == 0) *counter = 0u;
+}
+
 struct ReconTerms { double numel[CG_RECON_MAX_TERMS], w[CG_RECON_MAX_TERMS]; };
 
 // after the all-reduce: pub[k][g] = sums[k][g] / numel[k]; total[g] += sum_k w[k] * pub[k][g] through the double accumulator of
@@ -853,6 +924,24 @@ extern "C" int cg_recon_head_fwd(const float* h, const float* x, float* sums, in
     }
     launch_k(recon_head_fwd_kernel, nchunks * G, 256, 0, ST, h, x, sums, ws_part(ws), ws_counter(ws), G, npix, nchunks);
     return check_launch("recon_head_fwd");
+}
+
+extern "C" int cg_vgg_loss(const float* f_img, const float* mean_img, const float* rstd_img, const float* f_tgt, const float* mean_tgt,
+                           const float* rstd_tgt, int R, int B, int per_dir, int HW, int C, float coef, float* sums, float* d_pre, void* ws,
+                           size_t ws_bytes, void* stream) {
+    CG_REQUIRE(f_img && mean_img && rstd_img && f_tgt && mean_tgt && rstd_tgt && sums && d_pre, "vgg_loss: NULL argument");
+    CG_REQUIRE(R >= 1 && B >= 1 && per_dir >= B && per_dir % B == 0 && R % per_dir == 0 && HW >= 1 && C >= VL_CH && C % VL_CH == 0,
+               "vgg_loss: R=%d B=%d per_dir=%d HW=%d C=%d out of range", R, B, per_dir, HW, C);
+    const int nterm = R / B, nchunk = C / VL_CH;
+    CG_REQUIRE(nterm <= 256, "vgg_loss: %d terms (R / B) exceed 256", nterm);
+    const size_t need = 16 + CG_LOSS_MAX_G * 8 + (size_t)R * nchunk * 4;
+    if (need > ws_bytes) {
+        set_error("vgg_loss: workspace %zu < %zu bytes", ws_bytes, need);
+        return CG_ERR_WORKSPACE;
+    }
+    launch_k(vgg_loss_kernel, R * nchunk, 256, 0, ST, f_img, mean_img, rstd_img, f_tgt, mean_tgt, rstd_tgt, coef, d_pre, sums, ws_part(ws),
+             ws_counter(ws), B, per_dir, HW, C, nterm);
+    return check_launch("vgg_loss");
 }
 
 extern "C" int cg_recon_head_bwd(const float* h, const float* x, float coef, float* dh_pre, int G, int B, int HW, void* stream) {

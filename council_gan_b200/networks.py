@@ -737,3 +737,79 @@ class CouncilDis(_StackedNet):
                 pass
             dx = up
         return dx
+
+
+# ------------------------------------------------------------------------------------------------------
+# the frozen feature network of the perceptual loss (vgg_w)
+# ------------------------------------------------------------------------------------------------------
+class Vgg16:
+    """Vgg16 networks.py:573-622 up to relu5_3, frozen, for compute_vgg_loss (trainer_council.py:636-641).  One weight group (G = 1): the
+    trainer stacks every translation of every member and both directions into the batch of one pass.  The parameters are loaded from
+    the reference's ``vgg16.weight`` (a torch.save'd state_dict with keys conv{1_1..5_3}.{weight,bias}, utils.py:350-366); conv1_1's
+    3 input channels sit on lanes 0..2 of 4.  No gradient, optimiser state or checkpoint of its own: it is not one of the trainer's
+    networks."""
+
+    STAGES = ((('conv1_1', 3, 64), ('conv1_2', 64, 64)),
+              (('conv2_1', 64, 128), ('conv2_2', 128, 128)),
+              (('conv3_1', 128, 256), ('conv3_2', 256, 256), ('conv3_3', 256, 256)),
+              (('conv4_1', 256, 512), ('conv4_2', 512, 512), ('conv4_3', 512, 512)),
+              (('conv5_1', 512, 512), ('conv5_2', 512, 512), ('conv5_3', 512, 512)))
+    POOL_AFTER = ('conv1_2', 'conv2_2', 'conv3_3')  # F.max_pool2d(h, 2, 2) follows these (none after conv4_3)
+
+    def __init__(self, ops):
+        self.ops = ops
+        self.specs = [LayerSpec(k, cout, cin, 3, 1, 1, lanes=[0, 1, 2] if cin == 3 else None)
+                      for stage in self.STAGES for k, cin, cout in stage]
+        self.bank = ParamBank(ops, 1, [e for s in self.specs for e in s.entries()], trainable=False)
+
+    @staticmethod
+    def weight_path(vgg_model_path):
+        """where load_vgg16 (utils.py:350-366) reads the weights for hp['vgg_model_path'] (trainer_council.py:202)"""
+        import os
+        return os.path.join(vgg_model_path + '/models', 'vgg16.weight')
+
+    def load_state_dict(self, sd):
+        for s in self.specs:
+            s.import_weight(self.bank.p(s.wname)[0], sd[s.wname])
+            self.bank.p(s.bname)[0].copy_(sd[s.bname].detach().to('cpu', self.bank.data.dtype))
+
+    def load(self, vgg_model_path):
+        """Load <vgg_model_path>/models/vgg16.weight.  Never downloads or converts (the reference would fetch vgg16.t7 with wget)."""
+        import os
+        path = self.weight_path(vgg_model_path)
+        if not os.path.isfile(path):
+            raise FileNotFoundError('vgg_w needs the VGG-16 weights at %s (a torch.save\'d Vgg16 state_dict, as the reference\'s '
+                                    'load_vgg16 writes it); they are not downloaded' % path)
+        self.load_state_dict(torch.load(path, map_location='cpu'))
+        return self
+
+    def forward(self, x, saved=None):
+        """x [1,Bt,H,W,4]: preprocessed images (ops.vgg_preprocess) -> relu5_3 [1,Bt,H/8,W/8,512].  saved (a list): every ReLU output,
+        in layer order -- the masks of the data gradient and what the max-pool backward recomputes its windows from."""
+        ops, bank = self.ops, self.bank
+        h = x
+        for s in self.specs:
+            h = ops.conv_fwd(h, bank.p(s.wname), bank.p(s.bname), 1, 1, act=ACT_RELU)
+            if saved is not None:
+                saved.append(h)
+            if s.key in self.POOL_AFTER:
+                h = ops.maxpool2x2_fwd(h)
+        return h
+
+    def backward(self, d_pre, x_shape, saved):
+        """Data gradient only: d_pre = d(loss)/d(conv5_3's pre-activation) -> d(loss)/d(x) [1,Bt,H,W,4]."""
+        ops, bank = self.ops, self.bank
+        d = d_pre
+        for li in range(len(self.specs) - 1, -1, -1):
+            s = self.specs[li]
+            if li == 0:
+                return ops.conv_dgrad(d, bank.p(s.wname), x_shape, 1, 1)
+            prev = self.specs[li - 1]
+            if prev.key in self.POOL_AFTER:  # d(pool output), then through the pool and the previous layer's ReLU
+                pooled = saved[li - 1]
+                d = ops.conv_dgrad(d, bank.p(s.wname), (1,) + tuple(pooled.shape[1:2]) + (pooled.shape[2] // 2, pooled.shape[3] // 2,
+                                                                                          pooled.shape[4]), 1, 1)
+                d = ops.maxpool2x2_bwd(d, pooled)
+            else:
+                d = ops.conv_dgrad(d, bank.p(s.wname), saved[li - 1].shape, 1, 1, mask_src=saved[li - 1], mask_slope=0.0)
+        return d

@@ -95,6 +95,11 @@ _SIGS = {
                                     _fp]),
     'cg_recon_head_fwd': (C.c_int, [_fp, _fp, _fp, C.c_int, C.c_int, C.c_int, _fp, C.c_size_t, _fp]),
     'cg_recon_head_bwd': (C.c_int, [_fp, _fp, C.c_float, _fp, C.c_int, C.c_int, C.c_int, _fp]),
+    'cg_vgg_preprocess': (C.c_int, [_fp, _fp, C.c_long, _fp]),
+    'cg_vgg_preprocess_bwd': (C.c_int, [_fp, _fp, C.c_long, C.c_int, _fp]),
+    'cg_maxpool2x2_fwd': (C.c_int, [_fp, _fp] + [C.c_int] * 4 + [_fp]),
+    'cg_maxpool2x2_bwd': (C.c_int, [_fp, _fp, _fp] + [C.c_int] * 4 + [_fp]),
+    'cg_vgg_loss': (C.c_int, [_fp] * 6 + [C.c_int] * 5 + [C.c_float, _fp, _fp, _fp, C.c_size_t, _fp]),
     'cg_global_avgpool_fwd': (C.c_int, [_fp, _fp, C.c_int, C.c_int, C.c_int, _fp]),
     'cg_global_avgpool_bwd': (C.c_int, [_fp, _fp, _fp, C.c_int, C.c_int, C.c_int, C.c_int, _fp]),
     'cg_loss_workspace_bytes': (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int]),
@@ -749,6 +754,68 @@ class CudaOps:
                         lambda: self._ck(self.lib.cg_recon_head_bwd(_p(h), _p(x_in), float(coef), _p(dh), G, B, H * W, self._stream()),
                                          'cg_recon_head_bwd'))
         return dh
+
+    # -- perceptual loss (vgg_w): the frozen VGG-16's preprocessing, max-pools and loss ------------------------------------------------
+    def vgg_preprocess(self, x, out=None):
+        """vgg_preprocess (utils.py:380-390) of channels-last images [..., 4]: {B', G', R', 0}, c' = (x_c + 1) * 255 * 0.5 - mean_c.
+        out: a tensor of the same size to write into (default: a new one).  ONE launch."""
+        self._chk(x, out)
+        assert x.shape[-1] == 4
+        y = self.empty(*x.shape) if out is None else out
+        assert y.numel() == x.numel()
+        self._timed_raw('hbm:vgg_preprocess n%d' % x.numel(), 4.0 * 2 * x.numel(),
+                        lambda: self._ck(self.lib.cg_vgg_preprocess(_p(x), _p(y), x.numel() // 4, self._stream()), 'cg_vgg_preprocess'))
+        return y
+
+    def vgg_preprocess_bwd(self, dy, d_x, accumulate):
+        """d_x[..., c] (+)= 127.5 * dy[..., 2 - c] for c < 3 (lane 3: written 0, or kept when accumulating).  ONE launch."""
+        self._chk(dy, d_x)
+        assert dy.numel() == d_x.numel() and d_x.shape[-1] == 4
+        self._timed_raw('hbm:vgg_preprocess_bwd n%d' % dy.numel(), 4.0 * (3 if accumulate else 2) * dy.numel(),
+                        lambda: self._ck(self.lib.cg_vgg_preprocess_bwd(_p(dy), _p(d_x), dy.numel() // 4, int(bool(accumulate)),
+                                                                        self._stream()), 'cg_vgg_preprocess_bwd'))
+
+    def maxpool2x2_fwd(self, x):
+        """F.max_pool2d(x, 2, 2) of [G,B,H,W,C] (floor size) -> [G,B,H/2,W/2,C].  ONE launch."""
+        self._chk(x)
+        G, B, H, W, Cc = x.shape
+        y = self.empty(G, B, H // 2, W // 2, Cc)
+        self._timed_raw('hbm:maxpool2x2_fwd B%d %dx%d C%d' % (G * B, H, W, Cc), 4.0 * (x.numel() + y.numel()),
+                        lambda: self._ck(self.lib.cg_maxpool2x2_fwd(_p(x), _p(y), G * B, H, W, Cc, self._stream()), 'cg_maxpool2x2_fwd'))
+        return y
+
+    def maxpool2x2_bwd(self, dy, x):
+        """The gradient w.r.t. the pre-activation of x = relu(pre) [G,B,H,W,C] through max_pool2d(x, 2, 2), from dy [G,B,H/2,W/2,C]:
+        each window's first maximum takes dy where x > 0, every other position 0.  No index tensor.  ONE launch."""
+        self._chk(dy, x)
+        G, B, H, W, Cc = x.shape
+        assert tuple(dy.shape) == (G, B, H // 2, W // 2, Cc)
+        dx = self.empty(G, B, H, W, Cc)
+        self._timed_raw('hbm:maxpool2x2_bwd B%d %dx%d C%d' % (G * B, H, W, Cc), 4.0 * (2 * x.numel() + dy.numel()),
+                        lambda: self._ck(self.lib.cg_maxpool2x2_bwd(_p(dy), _p(x), _p(dx), G * B, H, W, Cc, self._stream()),
+                                         'cg_maxpool2x2_bwd'))
+        return dx
+
+    def vgg_loss(self, f_img, f_tgt, B, per_dir, coef, sums):
+        """compute_vgg_loss (trainer_council.py:636-641) of stacked relu5_3 rows f_img [1,R,h,w,C] against f_tgt [1,T,h,w,C], image row r
+        paired with target row (r // per_dir) * B + r % B: sums[k] = sum (IN(f_img) - IN(f_tgt))^2 over rows [k B, k B + B) on this rank
+        (R // B values); returns d(pre-activation of conv5_3) [1,R,h,w,C] of coef * that sum (the targets take no gradient).  The
+        statistics come from in_stats; the loss and its gradient are ONE more launch."""
+        self._chk(f_img, f_tgt, sums)
+        _, R, h, w, Cc = f_img.shape
+        assert f_tgt.shape[0] == 1 and tuple(f_tgt.shape[2:]) == (h, w, Cc) and sums.numel() == R // B
+        mi, ri = self.in_stats(f_img)
+        mt, rt = self.in_stats(f_tgt)
+        d_pre = self.empty(*f_img.shape)
+        need = 16 + 8 * LOSS_MAX_G + 4 * R * (Cc // 32)
+        if need > self._loss_ws.numel():
+            self._loss_ws = self._zero_bytes(need + 4096)
+        ws = self._loss_ws
+        self._timed_raw('hbm:vgg_loss R%d %dx%d C%d' % (R, h, w, Cc), 4.0 * (5 * f_img.numel()),
+                        lambda: self._ck(self.lib.cg_vgg_loss(_p(f_img), _p(mi), _p(ri), _p(f_tgt), _p(mt), _p(rt), R, B, per_dir, h * w, Cc,
+                                                              float(coef), _p(sums), _p(d_pre), _p(ws), ws.numel(), self._stream()),
+                                         'cg_vgg_loss'))
+        return d_pre
 
     # -- input pipeline (council_gan_b200/data.py) ------------------------------------------------------
     def aug_color(self, pix, desc, opcode, param, B, max_pixels, any_contrast):

@@ -58,8 +58,15 @@ What is different underneath (GPU-first, see DESIGN.md):
     gan_w != 0) gen_update draws one discriminator per member and runs D on a scratch bank whose member g holds discriminator
     dis_map[g]'s parameters (one gather launch per direction).  Under data parallelism every rank must seed numpy identically.  With
     all three off (the shipped configs) nothing of it runs and neither update draws from numpy.
-Paths outside the live configuration space of the reference's three configs (recon_x_cyc / vgg losses,
-nsgan/RaHinge, do_my_style, do_w_loss_matching_focus) raise NotImplementedError.
+  * vgg_w (:199-205, 531-538, 636-641, the perceptual loss; both directions required): the frozen VGG-16 is loaded from
+    <vgg_model_path>/models/vgg16.weight at construction (never downloaded).  After both forwards every translation of every member
+    and both directions is preprocessed into the batch of ONE VGG pass ([x_ab ; x_ba], one weight group), the targets [x_a ; x_b]
+    once per update, forward only.  One launch computes the sums of the instance-normalised squared error of relu5_3 (they join the
+    scalar all-reduce) and its gradient; the VGG data gradient runs before the per-direction backward, and its d(x_fake) joins d_x.
+    ``loss_gen_vgg_{a,b}_s`` are published through the reconstruction terms' finalize launch.  The network is not one of the
+    trainer's networks: no optimiser state, checkpoint or all-reduce.  With vgg_w 0 (the shipped configs) nothing of it runs.
+Paths outside the live configuration space of the reference's three configs (recon_x_cyc loss, nsgan/RaHinge, do_my_style,
+do_w_loss_matching_focus) raise NotImplementedError.
 """
 from __future__ import annotations
 
@@ -73,7 +80,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from .networks import IMG_C, CouncilDis, CouncilGen
+from .networks import IMG_C, CouncilDis, CouncilGen, Vgg16
 from .utils import get_model_list
 
 _DIRS = ('a2b', 'b2a')
@@ -192,6 +199,8 @@ class Council_Trainer(nn.Module):
             net._before_access = self._flush
             object.__setattr__(self, name + '_s', [net.member(i) for i in range(N)])
         self.style_dim = hp['gen']['style_dim']
+        # the frozen VGG-16 of the perceptual loss (:199-205): loaded once, on every rank, from the same file
+        self.vgg = Vgg16(_ops).load(hp['vgg_model_path']) if hp.get('vgg_w', 0) > 0 else None
 
         display_size = int(hp['display_size'])  # :136-138
         self.s_a = torch.randn(display_size, self.style_dim, 1, 1).to(_ops.device)
@@ -249,9 +258,14 @@ class Council_Trainer(nn.Module):
     # ------------------------------------------------------------------------------------------------
     @staticmethod
     def _check_supported(hp):
-        bad = [k for k in ('recon_x_cyc_w', 'vgg_w') if hp.get(k, 0) != 0]
+        bad = [k for k in ('recon_x_cyc_w',) if hp.get(k, 0) != 0]
         if bad:
             raise NotImplementedError('loss terms %s are not on the accelerated training path' % bad)
+        if hp.get('vgg_w', 0) != 0 and not (hp['do_a2b'] and hp['do_b2a']):
+            raise NotImplementedError('vgg_w compares both directions\' translations with their sources, so it needs do_a2b and do_b2a '
+                                      '(with one direction the reference fails with an IndexError)')
+        if hp.get('vgg_w', 0) < 0:
+            raise NotImplementedError('vgg_w must not be negative (the reference fails with an AttributeError on int.cuda)')
         if any(hp.get(k, 0) != 0 for k in ('recon_x_w', 'recon_c_w', 'recon_s_w')) and not (hp['do_a2b'] and hp['do_b2a']):
             raise NotImplementedError('recon_x_w / recon_c_w / recon_s_w decode or re-encode with the other direction\'s generator, so '
                                       'they need do_a2b and do_b2a (with one direction the reference fails with an IndexError)')
@@ -618,11 +632,16 @@ class Council_Trainer(nn.Module):
         recon = [(kind, dom, hp['recon_%s_w' % kind]) for kind in ('x', 's', 'c') if hp['recon_%s_w' % kind] != 0 for dom in ('a', 'b')]
         if (hp['recon_s_w'] != 0 or hp['recon_x_w'] != 0) and not all(self._nets['gen_' + d].sty_bank.trainable for d in self._dirs):
             raise NotImplementedError('recon_s_w / recon_x_w train the style encoder: they must be non-zero when the trainer is built')
+        vgg_w = hp['vgg_w']
+        if vgg_w != 0 and self.vgg is None:
+            raise NotImplementedError('vgg_w loads the VGG-16 when the trainer is built: it must be positive then')
+        # the terms of the finalize launch: the reconstructions, then the perceptual loss of x_ab (vgg_b) and of x_ba (vgg_a)
+        fin = recon + ([('vgg', 'b', vgg_w), ('vgg', 'a', vgg_w)] if vgg_w != 0 else [])
 
         # ---- forward of every direction; pass 1 of the loss (all reductions, one launch per direction) -----------
         fw = {}
         nd = len(self._dirs)
-        extra = (nd * N * 2 if be_on else 0) + (nd * N if ca_on else 0) + len(recon) * N
+        extra = (nd * N * 2 if be_on else 0) + (nd * N if ca_on else 0) + len(fin) * N
         if extra:  # the abs_beginning_end sums [|d|, d^2], the council abs sums and the recon sums ride behind the other scalars:
             red = ops.empty(nd * N * 6 + extra)  # still one all-reduce
             scal, off = red[:nd * N * 6].view(nd, N, 6), nd * N * 6
@@ -630,8 +649,8 @@ class Council_Trainer(nn.Module):
                 be_sums, off = red[off:off + nd * N * 2].view(nd, N, 2), off + nd * N * 2
             if ca_on:
                 ca_sums, off = red[off:off + nd * N].view(nd, N), off + nd * N
-            if recon:
-                rc_sums = red[off:].view(len(recon), N)
+            if fin:
+                rc_sums = red[off:].view(len(fin), N)
         else:
             red = scal = ops.empty(nd, N, 6)  # per direction and member: [adv, council, focus sums x4] of THIS rank
         for di, d in enumerate(self._dirs):
@@ -669,13 +688,18 @@ class Council_Trainer(nn.Module):
             if recon:
                 rec['c'], rec['src'] = c, src
             fw[d] = rec
-        if recon:
-            recon_numel = self._recon_forward(fw, s, recon, rc_sums)
+        fin_numel = self._recon_forward(fw, s, recon, rc_sums) if recon else []
+        if vgg_w != 0:
+            vgg_numel, vgg_rec = self._vgg_forward(fw, img_a, img_b, rc_sums[len(recon):], vgg_w)
+            fin_numel += [vgg_numel] * 2
         self._flush()  # (a family gated off above still steps here)
         dist = _dist()
         if dist is not None and self.world > 1:
             dist.all_reduce(red)  # sums over ranks; pass 2 divides the means by world and uses the GLOBAL (sum m / numel)^2
         d_x_re = self._recon_backward(fw, recon) if recon else {}
+        if vgg_w != 0:  # d(VGG input) of both directions, [1, 2NB, H, W, 4]
+            d_vgg = self.vgg.backward(*vgg_rec)
+            del vgg_rec
 
         # ---- pass 2 (loss assembly + history matching on the device, remaining loss gradients) and the backward ------
         total = ops.empty(N)
@@ -726,6 +750,12 @@ class Council_Trainer(nn.Module):
                     d_x = d_x_re[d]
                 else:
                     ops.add_(d_x, d_x_re[d])
+            if vgg_w != 0:  # through vgg_preprocess: d_x += 127.5 * the lane-swapped gradient of this direction's half of the batch
+                d_vd = d_vgg[0, di * N * rec['B']:(di + 1) * N * rec['B']]
+                fresh = d_x is None
+                if fresh:
+                    d_x = ops.empty(*rec['x_fake'].shape)
+                ops.vgg_preprocess_bwd(d_vd, d_x, accumulate=not fresh)
             if d_x is None:
                 d_x = ops.zeros(*rec['x_fake'].shape)
             if be_on:  # after gen_loss_bwd of this direction: the totals share its accumulator
@@ -741,9 +771,9 @@ class Council_Trainer(nn.Module):
                 ops.add_(gen.bank.grad[:gen.enc_end], gen.reencode_grad())
             if data_parallel:
                 self._reduce_async('gen', gen, 0, gen.enc_end)  # encoder bucket; the decoder bucket went out during the encoder backward
-        if recon:  # after every gen_loss_bwd / abs_beginning_end_bwd of this update: the member totals share their accumulator
-            rc_pub = ops.empty(len(recon), N)
-            ops.recon_finalize(rc_sums, recon_numel, [float(w) for _, _, w in recon], total, rc_pub)
+        if fin:  # after every gen_loss_bwd / abs_beginning_end_bwd of this update: the member totals share their accumulator
+            rc_pub = ops.empty(len(fin), N)
+            ops.recon_finalize(rc_sums, fin_numel, [float(w) for _, _, w in fin], total, rc_pub)
         if ca_on:  # :616-619: each direction's published council loss takes the OTHER direction's abs term (both directions are on)
             for di in range(nd):
                 ops.add_column(pub[di], 5, ca_pub[nd - 1 - di])
@@ -781,6 +811,9 @@ class Council_Trainer(nn.Module):
                     setattr(self, 'loss_gen_recon_%s_%s_s' % (kind, dom), [])
             for k, (kind, dom, _) in enumerate(recon):
                 setattr(self, 'loss_gen_recon_%s_%s_s' % (kind, dom), [rc_pub[k, i] for i in range(N)])
+        if vgg_w != 0:  # :531-536: one entry per member, vgg_a the b2a translation's term
+            self.loss_gen_vgg_b_s = [rc_pub[len(recon), i] for i in range(N)]
+            self.loss_gen_vgg_a_s = [rc_pub[len(recon) + 1, i] for i in range(N)]
         self._last_fw = {d: {'x_fake': fw[d]['x_fake'], 'mask': fw[d]['mask']} for d in self._dirs}
 
     def _dis_members(self, d, dis_map):
@@ -831,6 +864,29 @@ class Council_Trainer(nn.Module):
                 ops.latent_l1(s_rec, s[d], sums[k], float(w) / n, da=rec['d_s_rec'])
             numel.append(float(n))
         return numel
+
+    def _vgg_forward(self, fw, img_a, img_b, sums, w):
+        """The perceptual loss, compute_vgg_loss (:636-641) for every member and both directions in ONE VGG pass: the batch
+        [x_ab (N B) ; x_ba (N B)] keeps its ReLU outputs, the targets [x_a ; x_b] run once, forward only.  sums [2, N] = this rank's
+        sums of the squared error of x_ab against x_a (vgg_b) and of x_ba against x_b (vgg_a); their gradient w.r.t. conv5_3's
+        pre-activation is written in the same launch.  -> (numel of each term over the GLOBAL minibatch, arguments of Vgg16.backward)"""
+        ops, N = self.ops, self.council_size
+        xa, xb = fw['a2b']['x_fake'], fw['b2a']['x_fake']
+        assert xa.shape == xb.shape and img_a.shape == img_b.shape, 'vgg_w stacks both directions: their batches must have one shape'
+        _, B, H, W, _ = xa.shape
+        x = ops.empty(1, 2 * N * B, H, W, IMG_C)
+        ops.vgg_preprocess(xa, out=x[0, :N * B])
+        ops.vgg_preprocess(xb, out=x[0, N * B:])
+        tgt = ops.empty(1, 2 * B, H, W, IMG_C)
+        ops.vgg_preprocess(img_a, out=tgt[0, :B])
+        ops.vgg_preprocess(img_b, out=tgt[0, B:])
+        saved = []
+        f = self.vgg.forward(x, saved)
+        f_tgt = self.vgg.forward(tgt)
+        _, _, h, wd, Cf = f.shape
+        numel = float(B * self.world * Cf * h * wd)
+        d_pre = ops.vgg_loss(f, f_tgt, B, N * B, w / numel, sums)
+        return numel, (d_pre, x.shape, saved)
 
     def _recon_backward(self, fw, recon):
         """Backward of the reconstruction passes, before either generator's own backward.  recon_x: the other generator's decoder

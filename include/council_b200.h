@@ -265,7 +265,7 @@ int cg_council_abs_bwd(const float* x_fake, const int32_t* host_peer, int gray, 
  * coef = w / numel of the GLOBAL minibatch.  db needs a per-member b. */
 int cg_latent_l1(const float* a, const float* b, int b_shared, float* da, float* db, float coef, int accumulate, float* sums,
                  int G, long n, void* ws, size_t ws_bytes, void* stream);
-#define CG_RECON_MAX_TERMS 6
+#define CG_RECON_MAX_TERMS 8
 /* after the all-reduce of sums[nterm][G]: pub[k][g] = sums[k][g] / host_numel[k]; total[g] += sum_k host_weight[k] * pub[k][g]
  * through the double accumulator cg_gen_loss_bwd keeps in the same workspace (so it must follow the cg_gen_loss_bwd calls of
  * this update on that workspace and stream).  host_numel / host_weight (host memory) are passed by value. */
@@ -279,6 +279,30 @@ int cg_recon_finalize(const float* sums, const double* host_numel, const double*
 int cg_recon_head_fwd(const float* h, const float* x, float* sums, int G, int B, int HW, void* ws, size_t ws_bytes, void* stream);
 int cg_recon_head_bwd(const float* h, const float* x, float coef, float* dh_pre, int G, int B, int HW, void* stream);
 size_t cg_loss_workspace_bytes(int G, int B, int H, int W);
+
+/* ---- perceptual loss, vgg_w (trainer_council.py:199-205, 531-538, 636-641): the frozen Vgg16 (networks.py:573-622) runs on
+ *      cg_conv_fwd (CG_ACT_RELU) / cg_conv_dgrad (mask_src = the previous ReLU output, slope 0); these are the other pieces ---------- */
+/* vgg_preprocess (utils.py:380-390) on channels-last pixels x[npix][4] (lanes 0..2 RGB): y[npix][4] = {B', G', R', 0} with
+ * c' = (x_c + 1) * 255 * 0.5 - {103.939, 116.779, 123.680}[BGR lane], each operation rounded as torch rounds it */
+int cg_vgg_preprocess(const float* x, float* y, long npix, void* stream);
+/* its data gradient: d_x[p][c] (+)= 127.5 * dy[p][2 - c] for c = 0..2; lane 3 is written 0 (accumulate 0) or kept (accumulate 1) */
+int cg_vgg_preprocess_bwd(const float* dy, float* d_x, long npix, int accumulate, void* stream);
+/* F.max_pool2d(x, 2, 2) (networks.py:598, 603, 609), floor size: x[N][H][W][C] -> y[N][H/2][W/2][C], C % 4 == 0 */
+int cg_maxpool2x2_fwd(const float* x, float* y, int N, int H, int W, int C, void* stream);
+/* backward of max_pool2d(relu(pre)) w.r.t. pre, without an index tensor: x = the saved ReLU output [N][H][W][C]; each window's first
+ * maximum in row-major order (a later value must be strictly greater, as max_pool2d picks it) takes dy[N][H/2][W/2][C] where x > 0;
+ * every other position of dx[N][H][W][C], and the last row / column an odd size leaves uncovered, is written 0 */
+int cg_maxpool2x2_bwd(const float* dy, const float* x, float* dx, int N, int H, int W, int C, void* stream);
+/* compute_vgg_loss (trainer_council.py:636-641) over R stacked image rows f_img[R][HW][C] (relu5_3) against the target rows
+ * f_tgt[.][HW][C], image row r paired with target row (r / per_dir) * B + r % B; mean / rstd [rows][C] from cg_in_stats (eps 1e-5),
+ * IN(f) = (f - mean) * rstd (nn.InstanceNorm2d(512, affine=False), :121).
+ * sums[k] (k < R / B) = sum of (IN(f_img) - IN(f_tgt))^2 over rows [k B, k B + B) on this rank (float partials per block, added in
+ * double in a fixed order); d_pre[R][HW][C] = the instance-norm backward (statistics included) of 2 coef (IN(f_img) - IN(f_tgt)), times
+ * relu5_3's mask f_img > 0: the gradient w.r.t. conv5_3's pre-activation for a loss coef * sum, coef = vgg_w / numel of the GLOBAL
+ * minibatch.  The targets take no gradient.  ws: the loss workspace (16 + 64 + 4 R C / 32 bytes at least). */
+int cg_vgg_loss(const float* f_img, const float* mean_img, const float* rstd_img, const float* f_tgt, const float* mean_tgt,
+                const float* rstd_tgt, int R, int B, int per_dir, int HW, int C, float coef, float* sums, float* d_pre, void* ws,
+                size_t ws_bytes, void* stream);
 
 /* plumbing: p[0:bytes] = 0 on `stream` (cudaMemsetAsync; keeps framework fill kernels out of the launch list) */
 int cg_zero(void* p, size_t bytes, void* stream);
