@@ -8,7 +8,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libcouncil_b200.so')
-SOURCES = ['api.cu', 'conv_simt.cu', 'conv_tc.cu', 'norm.cu', 'pointwise.cu', 'losses.cu', 'head_fused.cu', 'conv_small.cu', 'augment.cu', 'vgg.cu']
+SOURCES = ['api.cu', 'conv_simt.cu', 'conv_tc.cu', 'norm.cu', 'pointwise.cu', 'losses.cu', 'head_fused.cu', 'conv_small.cu', 'augment.cu', 'vgg.cu', 'pad.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '--use_fast_math=false', '-Xcompiler', '-fPIC']
 

@@ -27,6 +27,20 @@ from .ops import ACT_LRELU, ACT_NONE, ACT_RELU, ACT_TANH
 IMG_C = 4  # image tensors carry 3 live lanes + 1 zero lane (16-byte pixels)
 
 
+def _pad_type(pad_type):
+    """True for reflect: the pad_type of a network's Conv2dBlocks (networks.py:470-474), 'zero' or 'reflect' on the accelerated path"""
+    assert pad_type in ('zero', 'reflect')
+    return pad_type == 'reflect'
+
+
+def _padded(ops, x, s, reflect, ups=False):
+    """-> (the input a layer's convolution reads, the pad it applies): under reflect a layer with pad > 0 reads
+    nn.ReflectionPad2d(pad) of x (of x nearest-upsampled x2 with ups) with pad 0, since the convolutions pad with zeros only"""
+    if reflect and s.pad > 0:
+        return ops.reflect_pad(x, s.pad, ups), 0
+    return x, s.pad
+
+
 # ------------------------------------------------------------------------------------------------------
 # parameter storage
 # ------------------------------------------------------------------------------------------------------
@@ -238,7 +252,8 @@ class CouncilGen(_StackedNet):
     def __init__(self, ops, hp, G, input_dim=3):
         g = hp['gen']
         assert not g['do_my_style'], 'do_my_style generators are outside the accelerated path'
-        assert g['pad_type'] == 'zero' and g['activ'] == 'relu'
+        assert g['activ'] == 'relu'
+        self.reflect = _pad_type(g['pad_type'])
         assert input_dim == 3 and g['num_of_mask_dim_to_add'] == 3, 'mask head kernel is specialised for RGB + 3 masks'
         self.ops, self.hp, self.G = ops, hp, G
         self.dim, self.style_dim, self.nd, self.nr, self.mlp_dim = g['dim'], g['style_dim'], g['n_downsample'], g['n_res'], g['mlp_dim']
@@ -399,10 +414,14 @@ class CouncilGen(_StackedNet):
         # loop is an order of magnitude longer than the epilogue and hides the reduction; a separate pass on the narrow
         # full-resolution layers, which are epilogue-bound
         wide = s.cout >= 128 and s.k * s.k * s.cin >= 1024
-        if wide:
-            y, mean, rstd = ops.conv_fwd_stats(x, w, s.stride, s.pad, ups=ups_in)
+        if self.reflect and s.pad > 0:  # the upsample goes into the padding pass, whose output the weight gradient reads
+            x, pad, ups_in = ops.reflect_pad(x, s.pad, ups_in), 0, False
         else:
-            y = ops.conv_fwd(x, w, None, s.stride, s.pad, ups=ups_in)
+            pad = s.pad
+        if wide:
+            y, mean, rstd = ops.conv_fwd_stats(x, w, s.stride, pad, ups=ups_in)
+        else:
+            y = ops.conv_fwd(x, w, None, s.stride, pad, ups=ups_in)
             mean, rstd = ops.in_stats(y)
         z = ops.norm_act_fwd(y, mean, rstd, adain, off, res, act, ups_out)
         if saved is not None:
@@ -413,12 +432,16 @@ class CouncilGen(_StackedNet):
         """Backward of _conv_norm: fills the weight gradient (in bank.grad, or in the flat buffer grad laid out like it), returns
         d(input).  With ups_out, dz has the upsampled shape and the 2x2 fan-in is summed while it is read."""
         ops = self.ops
-        x, y, mean, rstd = rec
+        x, y, mean, rstd = rec  # x: the padded input under reflect
         off = self.adain_off.get(s.key, 0)
         dy = ops.norm_act_bwd(dz, y, mean, rstd, adain, off, act, ups_out, d_adain)
-        ops.conv_wgrad(x, dy, self._gv(grad, s.wname), None, s.stride, s.pad)
+        reflect = self.reflect and s.pad > 0
+        pad = 0 if reflect else s.pad
+        ops.conv_wgrad(x, dy, self._gv(grad, s.wname), None, s.stride, pad)
         if not need_dx:
             return None
+        if reflect:
+            return ops.reflect_pad_bwd(ops.conv_dgrad(dy, self.bank.p(s.wname), x.shape, s.stride, 0), s.pad, addend=addend)
         return ops.conv_dgrad(dy, self.bank.p(s.wname), x.shape, s.stride, s.pad, addend=addend)
 
     # -- forward ---------------------------------------------------------------------------------------
@@ -469,7 +492,8 @@ class CouncilGen(_StackedNet):
                 # no-grad pass: the rest of the decoder (AdaIN + ReLU of this block, the three 1x1 head layers, mask compositing)
                 # is one kernel; the 64-channel full-resolution map is read once instead of making four HBM round trips
                 w, _ = self._w(b, sl)
-                y = ops.conv_fwd(x, w, None, b.stride, b.pad)
+                xb, pad = _padded(ops, x, b, self.reflect)
+                y = ops.conv_fwd(xb, w, None, b.stride, pad)
                 mean, rstd = ops.in_stats(y)
                 (w1, b1), (w2, b2), (w3, b3) = (self._w(s, sl) for s in self.head)
                 return ops.head_fused(y, mean, rstd, adain, self.adain_off[b.key], w1, b1, w2, b2, w3, b3, x_img)
@@ -585,11 +609,13 @@ class CouncilGen(_StackedNet):
         def wb(s):
             w, b = sb.p(s.wname), sb.p(s.bname)
             return (w, b) if sl is None else (w[sl:sl + 1], b[sl:sl + 1])
-        acts = [x]
+        acts = []  # the input of each layer (padded under reflect), then the last layer's output
         h = x
         for s in self.sty:
-            h = ops.conv_fwd(h, *wb(s), s.stride, s.pad, act=ACT_RELU)
+            h, pad = _padded(ops, h, s, self.reflect)
             acts.append(h)
+            h = ops.conv_fwd(h, *wb(s), s.stride, pad, act=ACT_RELU)
+        acts.append(h)
         # global average pool, then the 1x1 conv as a linear layer.  Training (saved) pools with the library's kernel, which
         # style_backward differentiates; the no-grad API path (encode(), sample()) keeps the tensor mean it has always used, so its
         # results are unchanged and op sets without the pool op can still serve it.
@@ -614,11 +640,17 @@ class CouncilGen(_StackedNet):
         d = ops.global_avgpool_bwd(d, acts[-1])  # gated by the last layer's ReLU
         for li in range(len(self.sty) - 1, -1, -1):
             s = self.sty[li]
-            ops.conv_wgrad(acts[li], d, gv(s.wname), gv(s.bname), s.stride, s.pad)
+            reflect = self.reflect and s.pad > 0
+            pad = 0 if reflect else s.pad
+            ops.conv_wgrad(acts[li], d, gv(s.wname), gv(s.bname), s.stride, pad)
             if li == 0 and not want_dx:
                 return None
-            d = ops.conv_dgrad(d, sb.p(s.wname), acts[li].shape, s.stride, s.pad, addend=addend if li == 0 else None,
+            add = addend if li == 0 else None
+            # the ReLU gate read from the padded input gates every copy of a pixel alike, so it stays in the data gradient
+            d = ops.conv_dgrad(d, sb.p(s.wname), acts[li].shape, s.stride, pad, addend=None if reflect else add,
                                mask_src=acts[li] if li > 0 else None, mask_slope=0.0)
+            if reflect:
+                d = ops.reflect_pad_bwd(d, s.pad, addend=add)
         return d
 
     def member_style_encode(self, i, x):
@@ -644,7 +676,8 @@ class CouncilDis(_StackedNet):
     def __init__(self, ops, hp, G, input_dim=3, council=False):
         dp = hp['dis']
         assert dp['gan_type'] == 'lsgan', 'only the LSGAN objective is on the accelerated path'
-        assert dp['norm'] == 'none' and dp['activ'] == 'lrelu' and dp['pad_type'] == 'zero'
+        assert dp['norm'] == 'none' and dp['activ'] == 'lrelu'
+        self.reflect = _pad_type(dp['pad_type'])
         assert input_dim == 3
         self.ops, self.hp, self.G, self.council = ops, hp, G, council
         self.num_scales, self.n_layer = dp['num_scales'], dp['n_layer']
@@ -688,13 +721,15 @@ class CouncilDis(_StackedNet):
         outs = []
         for sc, (layers, tail) in enumerate(self.scales):
             h = x
-            acts = [h]
+            acts = []  # the input of each layer (padded under reflect), then the output
             for s in layers:
-                h = ops.conv_fwd(h, bank.p(s.wname), bank.p(s.bname), s.stride, s.pad, act=ACT_LRELU, slope=0.2)
+                h, pad = _padded(ops, h, s, self.reflect)
                 acts.append(h)
+                h = ops.conv_fwd(h, bank.p(s.wname), bank.p(s.bname), s.stride, pad, act=ACT_LRELU, slope=0.2)
             for s in tail:
-                h = ops.conv_fwd(h, bank.p(s.wname), bank.p(s.bname), 1, 0)
                 acts.append(h)
+                h = ops.conv_fwd(h, bank.p(s.wname), bank.p(s.bname), 1, 0)
+            acts.append(h)
             outs.append(h)
             if saved is not None:
                 saved.append(acts)
@@ -716,14 +751,19 @@ class CouncilDis(_StackedNet):
             for li in range(len(allspecs) - 1, -1, -1):
                 s = allspecs[li]
                 a_in = acts[li]
+                reflect = self.reflect and s.pad > 0
+                pad = 0 if reflect else s.pad
                 if want_wgrad:
-                    ops.conv_wgrad(a_in, d, bank.g(s.wname), bank.g(s.bname), s.stride, s.pad)
+                    ops.conv_wgrad(a_in, d, bank.g(s.wname), bank.g(s.bname), s.stride, pad)
                 if li == 0 and not want_dx:
                     break
-                # a_in is the lrelu OUTPUT of layer li-1 when that layer is one of `layers`
+                # a_in is the lrelu OUTPUT of layer li-1 when that layer is one of `layers` (padded under reflect: the gate read from
+                # it gates every copy of a pixel alike)
                 masked = 1 <= li <= nl
-                d = ops.conv_dgrad(d, bank.p(s.wname), a_in.shape, s.stride, s.pad,
+                d = ops.conv_dgrad(d, bank.p(s.wname), a_in.shape, s.stride, pad,
                                    mask_src=a_in if masked else None, mask_slope=0.2)
+                if reflect:
+                    d = ops.reflect_pad_bwd(d, s.pad)
             if want_dx:
                 dx_scales.append(d)
         if not want_dx:

@@ -100,6 +100,8 @@ _SIGS = {
     'cg_maxpool2x2_fwd': (C.c_int, [_fp, _fp] + [C.c_int] * 4 + [_fp]),
     'cg_maxpool2x2_bwd': (C.c_int, [_fp, _fp, _fp] + [C.c_int] * 4 + [_fp]),
     'cg_vgg_loss': (C.c_int, [_fp] * 6 + [C.c_int] * 5 + [C.c_float, _fp, _fp, _fp, C.c_size_t, _fp]),
+    'cg_reflect_pad': (C.c_int, [_fp, _fp] + [C.c_int] * 6 + [_fp]),
+    'cg_reflect_pad_bwd': (C.c_int, [_fp, _fp, _fp, _fp, C.c_float] + [C.c_int] * 5 + [_fp]),
     'cg_global_avgpool_fwd': (C.c_int, [_fp, _fp, C.c_int, C.c_int, C.c_int, _fp]),
     'cg_global_avgpool_bwd': (C.c_int, [_fp, _fp, _fp, C.c_int, C.c_int, C.c_int, C.c_int, _fp]),
     'cg_loss_workspace_bytes': (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int]),
@@ -816,6 +818,34 @@ class CudaOps:
                                                               float(coef), _p(sums), _p(d_pre), _p(ws), ws.numel(), self._stream()),
                                          'cg_vgg_loss'))
         return d_pre
+
+    # -- reflection padding (pad_type: reflect) --------------------------------------------------------------------------------------
+    def reflect_pad(self, x, p, ups=False):
+        """nn.ReflectionPad2d(p) of x [G,B,H,W,C] (after a nearest x2 upsample with ups) -> [G,B,Hs+2p,Ws+2p,C], the input of a
+        pad-0 convolution.  Raises when p is not smaller than the (upsampled) map.  ONE launch."""
+        self._chk(x)
+        G, B, H, W, Cc = x.shape
+        Hs, Ws = (2 * H, 2 * W) if ups else (H, W)
+        xp = self.empty(G, B, Hs + 2 * p, Ws + 2 * p, Cc)
+        self._timed_raw('hbm:reflect_pad G%d B%d %dx%d C%d p%d%s' % (G, B, H, W, Cc, p, ' ups' if ups else ''), 4.0 * (x.numel() + xp.numel()),
+                        lambda: self._ck(self.lib.cg_reflect_pad(_p(x), _p(xp), G * B, H, W, Cc, p, int(bool(ups)), self._stream()),
+                                         'cg_reflect_pad'))
+        return xp
+
+    def reflect_pad_bwd(self, dxp, p, addend=None, mask_src=None, mask_slope=0.0):
+        """The data gradient through reflect_pad (no upsample): dxp [G,B,H+2p,W+2p,C] -> (fold + addend) * act'(mask_src)
+        [G,B,H,W,C], addend / mask_src as in conv_dgrad.  ONE launch."""
+        self._chk(dxp, addend, mask_src)
+        G, B, Hp, Wp, Cc = dxp.shape
+        H, W = Hp - 2 * p, Wp - 2 * p
+        dx = self.empty(G, B, H, W, Cc)
+        for t in (addend, mask_src):
+            assert t is None or tuple(t.shape) == tuple(dx.shape), (tuple(t.shape), tuple(dx.shape))
+        units = (dxp.numel() + dx.numel() * (1 + (addend is not None) + (mask_src is not None))) / dx.numel()
+        self._timed_raw('hbm:reflect_pad_bwd G%d B%d %dx%d C%d p%d' % (G, B, H, W, Cc, p), 4.0 * units * dx.numel(),
+                        lambda: self._ck(self.lib.cg_reflect_pad_bwd(_p(dxp), _p(dx), _p(addend), _p(mask_src), mask_slope, G * B, H, W, Cc,
+                                                                     p, self._stream()), 'cg_reflect_pad_bwd'))
+        return dx
 
     # -- input pipeline (council_gan_b200/data.py) ------------------------------------------------------
     def aug_color(self, pix, desc, opcode, param, B, max_pixels, any_contrast):

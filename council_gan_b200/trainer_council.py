@@ -65,6 +65,13 @@ What is different underneath (GPU-first, see DESIGN.md):
     scalar all-reduce) and its gradient; the VGG data gradient runs before the per-direction backward, and its d(x_fake) joins d_x.
     ``loss_gen_vgg_{a,b}_s`` are published through the reconstruction terms' finalize launch.  The network is not one of the
     trainer's networks: no optimiser state, checkpoint or all-reduce.  With vgg_w 0 (the shipped configs) nothing of it runs.
+  * pad_type: reflect (networks.py:463-520, ``gen.pad_type`` / ``dis.pad_type``; every shipped config documents zero/reflect): each
+    Conv2dBlock with a pad reads a reflect-padded copy of its input (cg_reflect_pad) through a convolution with pad 0, and the weight
+    gradient reads that copy, kept instead of the input.  The data gradient runs at the padded shape, and cg_reflect_pad_bwd folds the
+    reflected positions back and adds the residual gradient.  The no-grad decoder (encode / sample) pads the nearest-upsampled map in
+    the same pass instead of folding the upsample into the convolution.  The AvgPool pyramid, the MLP, the 1x1 layers and the VGG keep
+    zero padding; parameter names and checkpoints do not change.  Other pad types fail the networks' assertion.  With zero (the
+    shipped configs) nothing of it runs.
 Paths outside the live configuration space of the reference's three configs (recon_x_cyc loss, nsgan/RaHinge, do_my_style,
 do_w_loss_matching_focus) raise NotImplementedError.
 """

@@ -304,6 +304,19 @@ int cg_vgg_loss(const float* f_img, const float* mean_img, const float* rstd_img
                 const float* rstd_tgt, int R, int B, int per_dir, int HW, int C, float coef, float* sums, float* d_pre, void* ws,
                 size_t ws_bytes, void* stream);
 
+/* ---- reflection padding, pad_type: reflect (Conv2dBlock networks.py:470-471: nn.ReflectionPad2d(padding), then an nn.Conv2d with
+ *      padding 0).  The convolutions above pad with zeros only; a reflect layer runs cg_conv_* with pad 0 on the padded copy -------- */
+/* xp[N][Hs+2p][Ws+2p][C] = ReflectionPad2d(p) of x[N][H][W][C] (N = G*B), seen at Hs x Ws = H x W, or with ups = 1 at 2H x 2W
+ * nearest-upsampled first (nn.Upsample(scale_factor=2) networks.py:385, then the padding: one pass).  Index -i above the first row and
+ * 2 (Hs - 1) - i below the last: the edge pixel is not repeated.  C % 4 == 0; 1 <= p < Hs and p < Ws, as ReflectionPad2d requires. */
+int cg_reflect_pad(const float* x, float* xp, int N, int H, int W, int C, int p, int ups, void* stream);
+/* its backward: dx[N][H][W][C] = (fold(dxp) + addend) * act'(mask_src), fold(dxp) = the sum of every position of dxp[N][H+2p][W+2p][C]
+ * that the padding copied the pixel to (up to 9; 4 at the corners of a map larger than 2p), in padded row-major order.  addend /
+ * mask_src (shape of dx) may be NULL and mean what they mean in cg_conv_dgrad: act' = mask_src > 0 ? 1 : mask_slope.  No upsample:
+ * the x2 fan-in of an upsampled input is summed by cg_norm_act_bwd (ups) / cg_upsample2x_bwd.  1 <= p < H, p < W. */
+int cg_reflect_pad_bwd(const float* dxp, float* dx, const float* addend, const float* mask_src, float mask_slope, int N, int H, int W,
+                       int C, int p, void* stream);
+
 /* plumbing: p[0:bytes] = 0 on `stream` (cudaMemsetAsync; keeps framework fill kernels out of the launch list) */
 int cg_zero(void* p, size_t bytes, void* stream);
 
