@@ -133,6 +133,7 @@ extern "C" int cg_set_tensor_core_mode(int mode) {
     g_small_bn = ((mode >> 23) & 1) ? 0 : 1;  // bit 23: keep the widest N tile even when the launch has fewer tiles than SMs
     g_wgrad_tma = ((mode >> 25) & 1) ? 0 : 1;  // bit 25: stride-1 weight gradients on wgrad_tc_kernel instead of wgrad_tma_kernel
     g_pdl = (mode >> 22) & 1;  // bit 22: programmatic dependent launch
+    g_tc_serial_epilogue = (mode >> 26) & 1;  // bit 26: conv_tc_kernel's previous epilogue and tile walk
     return prev;
 }
 

@@ -16,6 +16,7 @@ extern std::atomic<uint64_t> g_launches;
 extern thread_local int g_tc_mode;
 extern thread_local int g_small_bn;
 extern thread_local int g_wgrad_tma;
+extern thread_local int g_tc_serial_epilogue;
 
 constexpr int CG_MAX_DEVICES = 64;
 inline int current_device() {

@@ -52,6 +52,7 @@ static int sm_count_now() {
     return g_sm_count_dev[dev];
 }
 thread_local int g_small_bn = 1;  // narrower N tiles when a launch has fewer tiles than SMs (mode bit 23 clears it)
+thread_local int g_tc_serial_epilogue = 0;  // mode bit 26 sets it: conv_tc_kernel's previous epilogue and tile walk, for comparisons
 static int g_driver_version = 0;
 static std::once_flag g_once;
 
@@ -157,9 +158,31 @@ struct TcParams {
     long stats_gbc;                 // G*B*Cout
     int act; float slope;
     int stages;
+    int serial_epilogue;            // mode bit 26: addend and mask loaded one column group and row at a time, classes walked outermost
 };
 
-// Persistent CTAs (one per SM) walk the tiles (group, class, N tile, pixel tile).  The producer thread streams (A, B) chunks
+// Tile t -> (pixel tile mt, N tile nt, class c, group g).  The classes of one pixel tile are neighbours in the walk, so the CTAs
+// running them at the same time read overlapping im2col boxes of the same activation tile and all but the first find it in L2
+// (class-outer, a stride-2 data gradient or upsample forward streams the whole activation from HBM once per class).
+__device__ __forceinline__ void tc_tile(const TcParams& p, int t, int MT, int NT, int& mt, int& nt, int& c, int& g) {
+    if (p.serial_epilogue) {
+        mt = t % MT;
+        int r = t / MT;
+        nt = r % NT;
+        r /= NT;
+        c = r % p.ncls;
+        g = r / p.ncls;
+        return;
+    }
+    c = t % p.ncls;
+    int r = t / p.ncls;
+    mt = r % MT;
+    r /= MT;
+    nt = r % NT;
+    g = r / NT;
+}
+
+// Persistent CTAs (one per SM) walk the tiles (group, N tile, pixel tile, class; see tc_tile).  The producer thread streams (A, B) chunks
 // through a ring of `stages` shared-memory slots guarded by full / empty mbarriers; each consumer warpgroup multiplies its 64
 // pixel rows of A with the whole B tile (wgmma, accumulators in registers), releases a slot as soon as the MMAs that read it
 // have retired, and runs the epilogue straight from registers while the producer already fills the slots of the next tile.
@@ -200,12 +223,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
             int stage = 0;
             uint32_t phase = 0;
             for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
-                int mt = t % MT;
-                int r = t / MT;
-                int nt = r % NT;
-                r /= NT;
-                int c = r % p.ncls;
-                int g = r / p.ncls;
+                int mt, nt, c, g;
+                tc_tile(p, t, MT, NT, mt, nt, c, g);
                 const TcClass& cl = p.cls[c];
                 long m0 = (long)mt * TC_BM;
                 int img = (int)(m0 / (p.P * p.Q));
@@ -245,12 +264,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
     int stage = 0;
     uint32_t phase = 0;
     for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
-        int mt = t % MT;
-        int r = t / MT;
-        int nt = r % NT;
-        r /= NT;
-        int c = r % p.ncls;
-        int g = r / p.ncls;
+        int mt, nt, c, g;
+        tc_tile(p, t, MT, NT, mt, nt, c, g);
         const TcClass& cl = p.cls[c];
         int prev = -1;
         for (int k0 = 0; k0 < kiters; k0 += p.cps) {
@@ -321,27 +336,63 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
             }
         }
         // each row's 8-column group is written by four consecutive lanes: 32 contiguous bytes, one full sector
+        if (!(p.addend || p.mask_src) || p.serial_epilogue) {
 #pragma unroll
-        for (int j = 0; j < BN / 8; j++) {
-            const int col = 8 * j + cq;
-            if (col >= p.n_store) break;
-            float2 bv = make_float2(0.f, 0.f);
-            if (p.bias) bv = __ldg(reinterpret_cast<const float2*>(p.bias + (long)g * p.Cout + nt * p.n_store + col));
+            for (int j = 0; j < BN / 8; j++) {
+                const int col = 8 * j + cq;
+                if (col >= p.n_store) break;
+                float2 bv = make_float2(0.f, 0.f);
+                if (p.bias) bv = __ldg(reinterpret_cast<const float2*>(p.bias + (long)g * p.Cout + nt * p.n_store + col));
 #pragma unroll
-            for (int h = 0; h < 2; h++) {
-                if (!valid[h]) continue;
-                float2 o = make_float2(acc[4 * j + 2 * h] + bv.x, acc[4 * j + 2 * h + 1] + bv.y);
-                if (p.addend) {
-                    const float2 a = __ldg(reinterpret_cast<const float2*>(p.addend + out_off[h] + col));
-                    o.x += a.x; o.y += a.y;
+                for (int h = 0; h < 2; h++) {
+                    if (!valid[h]) continue;
+                    float2 o = make_float2(acc[4 * j + 2 * h] + bv.x, acc[4 * j + 2 * h + 1] + bv.y);
+                    if (p.addend) {
+                        const float2 a = __ldg(reinterpret_cast<const float2*>(p.addend + out_off[h] + col));
+                        o.x += a.x; o.y += a.y;
+                    }
+                    if (p.mask_src) {
+                        const float2 a = __ldg(reinterpret_cast<const float2*>(p.mask_src + out_off[h] + col));
+                        o.x *= a.x > 0.f ? 1.f : p.slope; o.y *= a.y > 0.f ? 1.f : p.slope;
+                    } else if (p.act != CG_ACT_NONE) {
+                        o.x = apply_act(o.x, p.act, p.slope); o.y = apply_act(o.y, p.act, p.slope);
+                    }
+                    *reinterpret_cast<float2*>(p.y + out_off[h] + col) = o;
                 }
-                if (p.mask_src) {
-                    const float2 a = __ldg(reinterpret_cast<const float2*>(p.mask_src + out_off[h] + col));
-                    o.x *= a.x > 0.f ? 1.f : p.slope; o.y *= a.y > 0.f ? 1.f : p.slope;
-                } else if (p.act != CG_ACT_NONE) {
-                    o.x = apply_act(o.x, p.act, p.slope); o.y = apply_act(o.y, p.act, p.slope);
+            }
+            continue;
+        }
+        // Data gradient with a residual addend and / or an activation mask (no bias, no activation: tc_conv_dgrad never sets
+        // them).  The compiler cannot prove that y aliases neither operand, so in the loop above it keeps every load behind the
+        // previous store: a tile waits for BN / 4 global round trips in a row while the tensor cores idle.  Here the operands of
+        // EB column groups are all loaded before the first of their results is stored: one round trip per batch.  EB is bounded
+        // by the registers left beside the BN / 2 accumulators.
+        constexpr int EB = BN == 256 ? 2 : BN / 8 < 8 ? BN / 8 : 8;
+#pragma unroll
+        for (int j0 = 0; j0 < BN / 8; j0 += EB) {
+            float2 av[EB][2], mv[EB][2];
+#pragma unroll
+            for (int jj = 0; jj < EB; jj++) {
+                const int col = 8 * (j0 + jj) + cq;
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    const bool ld = col < p.n_store && valid[h];
+                    av[jj][h] = p.addend && ld ? __ldg(reinterpret_cast<const float2*>(p.addend + out_off[h] + col)) : make_float2(0.f, 0.f);
+                    mv[jj][h] = p.mask_src && ld ? __ldg(reinterpret_cast<const float2*>(p.mask_src + out_off[h] + col)) : make_float2(0.f, 0.f);
                 }
-                *reinterpret_cast<float2*>(p.y + out_off[h] + col) = o;
+            }
+#pragma unroll
+            for (int jj = 0; jj < EB; jj++) {
+                const int j = j0 + jj, col = 8 * j + cq;
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    if (col >= p.n_store || !valid[h]) continue;
+                    // + 0: the zero bias of the loop above, which turns an accumulator of -0 into +0
+                    float2 o = make_float2(acc[4 * j + 2 * h] + 0.f, acc[4 * j + 2 * h + 1] + 0.f);
+                    if (p.addend) { o.x += av[jj][h].x; o.y += av[jj][h].y; }
+                    if (p.mask_src) { o.x *= mv[jj][h].x > 0.f ? 1.f : p.slope; o.y *= mv[jj][h].y > 0.f ? 1.f : p.slope; }
+                    *reinterpret_cast<float2*>(p.y + out_off[h] + col) = o;
+                }
             }
         }
     }
@@ -468,6 +519,7 @@ static int launch_tc(TcParams& p, cudaStream_t st) {
     if (stages > 4 && stage_bytes >= 48 * 1024) stages = 4;
     if (p.n_store == 0) p.n_store = p.bn;
     p.stages = stages;
+    p.serial_epilogue = g_tc_serial_epilogue;
     size_t smem = (size_t)stages * stage_bytes + 1024 /*align slack*/ + 2 * stages * 8;
     void (*kern)(TcParams) = p.bk == 32 ? tc_kernel_for<32>(p.bn) : tc_kernel_for<8>(p.bn);
     if (!kern) {

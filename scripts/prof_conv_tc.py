@@ -3,9 +3,12 @@ launches of the step, at their production shapes.
 
     python scripts/prof_conv_tc.py [iters]
 
-CUDA events over `iters` (default 20) launches after warm-up, best of three rounds.  Prints ms per launch, algorithmic TFLOP/s
-and its ratio to the TF32 cuBLAS rate measured in the same process (torch.matmul 8192^3, best of 10, as bench.py measures it),
-and the card it ran on with its power limit."""
+CUDA events over `iters` (default 20) launches after warm-up.  Every launch runs with the default epilogue and tile walk and with
+the previous ones (mode bit 26), alternating three times in one process; the best of the three is reported for each.  Prints ms per
+launch, algorithmic TFLOP/s and its ratio to the TF32 cuBLAS rate measured in the same process (torch.matmul 8192^3, best of 10, as
+bench.py measures it), and the card it ran on with its power limit.  Epilogues as in the training step: the forward of the
+generator layers with the fused statistics, of the discriminator layers with bias and LeakyReLU; the data gradient of the
+discriminator layers masked by the layer input, of the residual layer with the residual addend."""
 import os
 import subprocess
 import sys
@@ -55,6 +58,9 @@ def timed(fn, iters):
     return e0.elapsed_time(e1) / iters
 
 
+MODES = [('default', 1), ('bit 26', 7 | (1 << 26))]
+
+
 def main():
     iters = int(sys.argv[1]) if len(sys.argv) > 1 else 20
     ops = CudaOps('cuda:0')
@@ -68,21 +74,28 @@ def main():
         gen = torch.Generator().manual_seed(0)
         x = torch.randn(G, B, H, W, Cin, generator=gen).cuda()
         w = (torch.randn(G, Cout, K, K, Cin, generator=gen) / (K * K * Cin) ** 0.5).cuda()
+        b = torch.randn(G, Cout, generator=gen).cuda()
         dy = torch.randn(G, B, Ho, Wo, Cout, generator=gen).cuda()
         flops = 2.0 * G * B * Ho * Wo * Cout * K * K * Cin
         if s == 1:  # generator layers feed instance norm / AdaIN: statistics in the epilogue
             fwd = lambda: ops.conv_fwd_stats(x, w, s, pad)[0]
-            dgrad = lambda: ops.conv_dgrad(dy, w, x.shape, s, pad)
-        else:  # discriminator layers: LeakyReLU 0.2
-            fwd = lambda: ops.conv_fwd(x, w, None, s, pad, act=ACT_LRELU, slope=0.2)
+            dgrad = lambda: ops.conv_dgrad(dy, w, x.shape, s, pad, addend=x if label == 'gen residual' else None)
+        else:  # discriminator layers: bias and LeakyReLU 0.2
+            fwd = lambda: ops.conv_fwd(x, w, b, s, pad, act=ACT_LRELU, slope=0.2)
             dgrad = lambda: ops.conv_dgrad(dy, w, x.shape, s, pad, mask_src=x, mask_slope=0.2)
         for kind, fn in (('fwd', fwd), ('dgrad', dgrad)):
-            times = [timed(fn, iters) for _ in range(3)]
-            t = min(times)
-            print('%-12s %-5s %dx%d s%d %d->%d %dx%d G%d B%d (%.1f GFLOP): %s ms, %.0f TFLOP/s, %.2f of cuBLAS'
-                  % (label, kind, K, K, s, Cin, Cout, H, W, G, B, flops / 1e9, ' '.join('%.3f' % v for v in times), flops / t / 1e9,
-                     flops / t / 1e9 / lib), flush=True)
-        del x, w, dy
+            times = {m: [] for _, m in MODES}
+            for _ in range(3):
+                for _, m in MODES:
+                    ops.set_tensor_core_mode(m)
+                    times[m].append(timed(fn, iters))
+            ops.set_tensor_core_mode(1)
+            for name, m in MODES:
+                t = min(times[m])
+                print('%-12s %-5s %dx%d s%d %d->%d %dx%d G%d B%d (%.1f GFLOP) %-8s: %s ms, %.0f TFLOP/s, %.2f of cuBLAS'
+                      % (label, kind, K, K, s, Cin, Cout, H, W, G, B, flops / 1e9, name, ' '.join('%.3f' % v for v in times[m]),
+                         flops / t / 1e9, flops / t / 1e9 / lib), flush=True)
+        del x, w, b, dy
         torch.cuda.empty_cache()
 
 
