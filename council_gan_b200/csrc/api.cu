@@ -134,6 +134,7 @@ extern "C" int cg_set_tensor_core_mode(int mode) {
     g_wgrad_tma = ((mode >> 25) & 1) ? 0 : 1;  // bit 25: stride-1 weight gradients on wgrad_tc_kernel instead of wgrad_tma_kernel
     g_pdl = (mode >> 22) & 1;  // bit 22: programmatic dependent launch
     g_tc_serial_epilogue = (mode >> 26) & 1;  // bit 26: conv_tc_kernel's previous epilogue and tile walk
+    g_tc_reg_epilogue = (mode >> 27) & 1;  // bit 27: conv_tc_kernel's register epilogue everywhere (no shared-memory / TMA epilogue)
     return prev;
 }
 

@@ -17,6 +17,7 @@ extern thread_local int g_tc_mode;
 extern thread_local int g_small_bn;
 extern thread_local int g_wgrad_tma;
 extern thread_local int g_tc_serial_epilogue;
+extern thread_local int g_tc_reg_epilogue;
 
 constexpr int CG_MAX_DEVICES = 64;
 inline int current_device() {

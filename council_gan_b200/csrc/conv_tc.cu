@@ -43,7 +43,9 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
 typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                    const int*, const int*, cuuint32_t, cuuint32_t, const cuuint32_t*, CUtensorMapInterleave,
                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+typedef CUresult (*ReplaceAddressFn)(CUtensorMap*, void*);
 static EncodeTiledFn g_encode_tiled = nullptr;
+static ReplaceAddressFn g_replace_address = nullptr;
 static EncodeIm2colFn g_encode_im2col = nullptr;
 static int g_sm_count_dev[CG_MAX_DEVICES] = {0};  // multiprocessors per device ordinal
 static int sm_count_now() {
@@ -53,6 +55,7 @@ static int sm_count_now() {
 }
 thread_local int g_small_bn = 1;  // narrower N tiles when a launch has fewer tiles than SMs (mode bit 23 clears it)
 thread_local int g_tc_serial_epilogue = 0;  // mode bit 26 sets it: conv_tc_kernel's previous epilogue and tile walk, for comparisons
+thread_local int g_tc_reg_epilogue = 0;     // mode bit 27 sets it: every conv_tc_kernel launch on the register epilogue, for comparisons
 static int g_driver_version = 0;
 static std::once_flag g_once;
 
@@ -120,6 +123,9 @@ static void init_driver() {
         fn = nullptr;
         if (cudaGetDriverEntryPoint("cuTensorMapEncodeIm2col", &fn, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
             g_encode_im2col = (EncodeIm2colFn)fn;
+        fn = nullptr;
+        if (cudaGetDriverEntryPoint("cuTensorMapReplaceAddress", &fn, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
+            g_replace_address = (ReplaceAddressFn)fn;
         cudaDriverGetVersion(&g_driver_version);
     });
 }
@@ -159,6 +165,10 @@ struct TcParams {
     int act; float slope;
     int stages;
     int serial_epilogue;            // mode bit 26: addend and mask loaded one column group and row at a time, classes walked outermost
+    // shared-memory epilogue (epi_slots > 0, chosen in launch_tc): 5-D tiled fp32 maps of y, the addend and the mask
+    // (encode_out_map), a ring of epi_slots slots of epi_slot_bytes holding one 32-channel column slice of a tile
+    CUtensorMap ymap, addmap, maskmap;
+    int epi_slots, epi_slot_bytes;
 };
 
 // Tile t -> (pixel tile mt, N tile nt, class c, group g).  The classes of one pixel tile are neighbours in the walk, so the CTAs
@@ -182,6 +192,18 @@ __device__ __forceinline__ void tc_tile(const TcParams& p, int t, int MT, int NT
     g = r / NT;
 }
 
+// Coordinates in the 5-D view of the output (encode_out_map) of the 64 pixels h * 64 .. h * 64 + 63 of pixel tile mt: q = column
+// of the first pixel in the class grid, n = image row index (g * B + img) * out_H / out_sh + row.  The shared-memory epilogue
+// serves P * Q % 128 == 0 and (Q % 64 == 0 or 64 % Q == 0) only, so the 64 pixels are one row segment or whole rows of one image.
+__device__ __forceinline__ void tc_half_coords(const TcParams& p, int g, int mt, int h, int& q, int& n) {
+    const int pq = p.P * p.Q;
+    const int m = mt * TC_BM + 64 * h;
+    const int img = m / pq, rem = m - img * pq;
+    const int pp = rem / p.Q;
+    q = rem - pp * p.Q;
+    n = (g * p.B + img) * (p.out_H / p.out_sh) + pp;
+}
+
 // Persistent CTAs (one per SM) walk the tiles (group, N tile, pixel tile, class; see tc_tile).  The producer thread streams (A, B) chunks
 // through a ring of `stages` shared-memory slots guarded by full / empty mbarriers; each consumer warpgroup multiplies its 64
 // pixel rows of A with the whole B tile (wgmma, accumulators in registers), releases a slot as soon as the MMAs that read it
@@ -196,8 +218,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
     constexpr int b_bytes = ((BN * BK * 4) + 1023) & ~1023;     // one K chunk of B (slot size)
     const int stage_bytes = p.cps * (a_bytes + b_bytes);         // [A_0..A_cps-1][B_0..B_cps-1]
     constexpr int tx_chunk = a_bytes + BN * BK * 4;
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * stage_bytes);
+    constexpr bool tma_epi = BK == 32 && BN >= 64;  // the host sets epi_slots only for these instantiations
+    const int epi_slots = tma_epi ? p.epi_slots : 0;
+    uint8_t* epi = smem + (size_t)p.stages * stage_bytes;  // epilogue ring, 1024-byte aligned (stage_bytes is a multiple of 1024)
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi + (size_t)epi_slots * p.epi_slot_bytes);
     uint64_t* empty_bar = full_bar + p.stages;
+    uint64_t* efull_bar = empty_bar + p.stages;
+    uint64_t* eempty_bar = efull_bar + epi_slots;
 
     const int MT = (p.B * p.P * p.Q + TC_BM - 1) / TC_BM;  // pixel tiles per (group, class)
     const int NT = (p.Cout + BN - 1) / BN;
@@ -211,6 +238,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
         for (int s = 0; s < p.stages; s++) {
             mbar_init(&full_bar[s], 1);
             mbar_init(&empty_bar[s], 2);  // one arrival per consumer warpgroup
+        }
+        if (epi_slots) {
+            prefetch_tmap(&p.ymap);
+            if (p.addend) prefetch_tmap(&p.addmap);
+            if (p.mask_src) prefetch_tmap(&p.maskmap);
+        }
+        for (int s = 0; s < epi_slots; s++) {
+            mbar_init(&efull_bar[s], 1);
+            mbar_init(&eempty_bar[s], 2);  // one arrival per consumer warpgroup
         }
         fence_barrier_init();
     }
@@ -250,6 +286,38 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
                     if (++stage == p.stages) { stage = 0; phase ^= 1; }
                 }
             }
+        } else if (tid == 32 && epi_slots) {
+            // epilogue operands: the addend and mask slices of each tile's output region, one 32-channel slice per ring slot, each
+            // as two 64-pixel boxes (one per consumer warpgroup).  Runs ahead of the consumers by the ring depth, i.e. during the
+            // main loop of the tile; without operands the slot is only handed over as staging for the output.
+            const uint32_t ebytes = (p.addend ? 2 * 8192 : 0) + (p.mask_src ? 2 * 8192 : 0);
+            int es = 0;
+            uint32_t ephase = 0;
+            for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+                int mt, nt, c, g;
+                tc_tile(p, t, MT, NT, mt, nt, c, g);
+                const TcClass& cl = p.cls[c];
+                int q[2], n[2];
+                tc_half_coords(p, g, mt, 0, q[0], n[0]);
+                tc_half_coords(p, g, mt, 1, q[1], n[1]);
+                for (int sl = 0; sl < BN / 32; sl++) {
+                    mbar_wait(&eempty_bar[es], ephase ^ 1);
+                    if (ebytes) {
+                        mbar_expect_tx(&efull_bar[es], ebytes);
+                        uint8_t* dst = epi + (size_t)es * p.epi_slot_bytes;
+                        const int c0 = nt * BN + 32 * sl;
+                        for (int h = 0; h < 2; h++) {
+                            if (p.addend) tma_load_5d(&p.addmap, &efull_bar[es], dst + h * 8192, c0, cl.out_w0, q[h], cl.out_h0, n[h]);
+                            if (p.mask_src)
+                                tma_load_5d(&p.maskmap, &efull_bar[es], dst + (p.addend ? 16384 : 0) + h * 8192, c0, cl.out_w0, q[h],
+                                            cl.out_h0, n[h]);
+                        }
+                    } else {
+                        mbar_arrive(&efull_bar[es]);
+                    }
+                    if (++es == epi_slots) { es = 0; ephase ^= 1; }
+                }
+            }
         }
         return;
     }
@@ -263,6 +331,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
     float acc[BN / 2];
     int stage = 0;
     uint32_t phase = 0;
+    int es = 0;
+    uint32_t ephase = 0;
     for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
         int mt, nt, c, g;
         tc_tile(p, t, MT, NT, mt, nt, c, g);
@@ -335,6 +405,67 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
                 if (lane < 16) st[16 * j] = v;
             }
         }
+        if constexpr (tma_epi) {
+            if (epi_slots) {
+                // Shared-memory epilogue, one 32-channel column slice at a time: combine the accumulators with the slice's operands,
+                // which the operand thread loaded during the main loop, write the result over the first operand (or into the empty
+                // slot), and store this warpgroup's 64 x 32 half with one TMA store.  Same operations per element, in the same
+                // order, as the register epilogue below.  The slot goes back to the operand thread once the store has read it.
+                int q, n;
+                tc_half_coords(p, g, mt, cw, q, n);
+                const int r0 = warp4 * 16 + (lane >> 2);  // this thread's rows of the warpgroup's 64-pixel half: r0, r0 + 8
+#pragma unroll
+                for (int sl = 0; sl < BN / 32; sl++) {
+                    float2 bv[4];
+#pragma unroll
+                    for (int jj = 0; jj < 4; jj++)
+                        bv[jj] = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + (long)g * p.Cout + nt * BN + 32 * sl + 8 * jj + cq))
+                                        : make_float2(0.f, 0.f);
+                    mbar_wait(&efull_bar[es], ephase);
+                    uint8_t* half = epi + (size_t)es * p.epi_slot_bytes + cw * 8192;  // [64 pixels][32 channels], 128-byte swizzle
+                    const uint8_t* msk = half + (p.addend ? 16384 : 0);
+#pragma unroll
+                    for (int jj = 0; jj < 4; jj++) {
+                        const int j = 4 * sl + jj;
+#pragma unroll
+                        for (int h = 0; h < 2; h++) {
+                            const int r = r0 + 8 * h;
+                            const int off = r * 128 + (((2 * jj + (cq >> 2)) ^ (r & 7)) << 4) + (cq & 3) * 4;
+                            float2 o = make_float2(acc[4 * j + 2 * h] + bv[jj].x, acc[4 * j + 2 * h + 1] + bv[jj].y);
+                            if (p.addend) {
+                                const float2 a = *reinterpret_cast<const float2*>(half + off);
+                                o.x += a.x; o.y += a.y;
+                            }
+                            if (p.mask_src) {
+                                const float2 a = *reinterpret_cast<const float2*>(msk + off);
+                                o.x *= a.x > 0.f ? 1.f : p.slope; o.y *= a.y > 0.f ? 1.f : p.slope;
+                            } else if (p.act != CG_ACT_NONE) {
+                                o.x = apply_act(o.x, p.act, p.slope); o.y = apply_act(o.y, p.act, p.slope);
+                            }
+                            *reinterpret_cast<float2*>(half + off) = o;
+                        }
+                    }
+                    fence_proxy_async();  // the generic-proxy writes above are visible to the TMA store
+                    named_bar_sync(1 + cw, 128);
+                    if (tid == 0) {
+                        tma_store_5d(&p.ymap, half, nt * BN + 32 * sl, cl.out_w0, q, cl.out_h0, n);
+                        bulk_commit();
+                        // hand back the previous slice's slot once its store has read it (this one's is still in flight); the
+                        // last slice of the tile waits for its own, so that the next tile's operands can be loaded during its main loop
+                        if (sl > 0) {
+                            bulk_wait_read<1>();
+                            mbar_arrive(&eempty_bar[es == 0 ? epi_slots - 1 : es - 1]);
+                        }
+                        if (sl == BN / 32 - 1) {
+                            bulk_wait_read<0>();
+                            mbar_arrive(&eempty_bar[es]);
+                        }
+                    }
+                    if (++es == epi_slots) { es = 0; ephase ^= 1; }
+                }
+                continue;
+            }
+        }
         // each row's 8-column group is written by four consecutive lanes: 32 contiguous bytes, one full sector
         if (!(p.addend || p.mask_src) || p.serial_epilogue) {
 #pragma unroll
@@ -396,6 +527,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
             }
         }
     }
+    if (epi_slots && tid == 0) bulk_wait<0>();  // the TMA stores of y have completed before the CTA exits
 }
 
 
@@ -458,6 +590,38 @@ static int encode_act_map(CUtensorMap* map, const float* x, long N, int H, int W
     return cached_map(map, k, [&](CUtensorMap* m) { return encode_act_map_raw(m, x, N, H, W, C, lo_w, lo_h, up_w, up_h, stride, bk); });
 }
 
+// Output-shaped tensor [NI][H][W][C] (y, the addend, the mask) for the shared-memory epilogue, viewed as 5-D (C, sw, W / sw, sh,
+// NI * H / sh): pixel (p, q) of the output class (h0, w0) with strides (sh, sw) is (c, w0, q, h0, n * H / sh + p), so the class
+// strides are plain coordinates and no TMA traversal stride is involved.  Box: 32 channels (one 128-byte swizzled row) x 64
+// pixels, qbox of one row x 64 / qbox rows.  FLOAT32: the values move raw, unlike the TF32 operand maps.  The descriptor is cached
+// by geometry alone and pointed at `t` by cuTensorMapReplaceAddress: outputs are often fresh allocations (a layer's y is), and
+// replacing the address costs far less than an encode.
+static int encode_out_map(CUtensorMap* map, const float* t, long NI, int H, int W, int C, int sh, int sw, int qbox) {
+    MapKey k{};
+    k.ptr = nullptr; k.a = NI; k.b = ((int64_t)H << 32) | (uint32_t)W;
+    k.v[0] = C; k.v[1] = sh; k.v[2] = sw; k.v[3] = qbox; k.v[7] = 3;
+    if (int rc = cached_map(map, k, [&](CUtensorMap* m) {
+            cuuint64_t dims[5] = {(cuuint64_t)C, (cuuint64_t)sw, (cuuint64_t)(W / sw), (cuuint64_t)sh, (cuuint64_t)(NI * H / sh)};
+            cuuint64_t strides[4] = {(cuuint64_t)C * 4, (cuuint64_t)sw * C * 4, (cuuint64_t)W * C * 4, (cuuint64_t)sh * W * C * 4};
+            cuuint32_t box[5] = {32, 1, (cuuint32_t)qbox, 1, (cuuint32_t)(64 / qbox)};
+            cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+            CUresult r = g_encode_tiled(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, (void*)t, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+            if (r != CUDA_SUCCESS) {
+                set_error("cuTensorMapEncodeTiled(output NI=%ld H=%d W=%d C=%d strides %d,%d box q %d) failed: %d", NI, H, W, C, sh, sw, qbox, (int)r);
+                return CG_ERR_CUDA;
+            }
+            return CG_OK;
+        }))
+        return rc;
+    CUresult r = g_replace_address(map, (void*)t);
+    if (r != CUDA_SUCCESS) {
+        set_error("cuTensorMapReplaceAddress(output NI=%ld H=%d W=%d C=%d) failed: %d", NI, H, W, C, (int)r);
+        return CG_ERR_CUDA;
+    }
+    return CG_OK;
+}
+
 static int pick_bn(int cout) {
     if (cout % 256 == 0) return 256;
     if (cout == 128) return 128;
@@ -507,9 +671,10 @@ static void (*tc_kernel_for(int bn))(TcParams) {
 static int launch_tc(TcParams& p, cudaStream_t st) {
     int a_bytes = TC_BM * p.bk * 4, b_bytes = ((p.bn * p.bk * 4) + 1023) & ~1023;
     int chunk_bytes = a_bytes + b_bytes;
-    // several K chunks per stage when a chunk carries little tensor work (N <= 128 or 32-byte rows): fewer barrier round trips
+    // several K chunks per stage when a chunk carries little tensor work (N <= 64 or 32-byte rows): fewer barrier round trips.  At
+    // N = 128 one chunk per stage (6 or 7 stages of 32 KB instead of 3 of 64 KB) measured 8-18 % faster on the production launches.
     int kiters = p.KH * p.KW * ((p.Cin + p.bk - 1) / p.bk);
-    int cps = p.bn <= 128 ? 2 : 1;
+    int cps = p.bn <= 64 ? 2 : 1;
     if (p.bk == 8) cps = 8;          // 6 KB chunks
     while (cps > 1 && (cps > kiters || cps * chunk_bytes > 64 * 1024)) cps >>= 1;
     p.cps = cps;
@@ -518,9 +683,33 @@ static int launch_tc(TcParams& p, cudaStream_t st) {
     if (stages > TC_MAX_STAGES) stages = TC_MAX_STAGES;
     if (stages > 4 && stage_bytes >= 48 * 1024) stages = 4;
     if (p.n_store == 0) p.n_store = p.bn;
-    p.stages = stages;
     p.serial_epilogue = g_tc_serial_epilogue;
-    size_t smem = (size_t)stages * stage_bytes + 1024 /*align slack*/ + 2 * stages * 8;
+    // Shared-memory epilogue (TMA-loaded operands, TMA-stored results) where each 64-pixel half tile is a row segment or whole rows
+    // of one image (tc_half_coords) and at least two ring slots fit beside the stages; elsewhere the register epilogue.  Slot: one
+    // 16 KB [128 pixels][32 channels] slice per operand (the result overwrites the first), or a bare staging slice.
+    p.epi_slots = 0;
+    const int nops = (p.addend ? 1 : 0) + (p.mask_src ? 1 : 0);
+    const bool aligned = ((uintptr_t)p.y | (uintptr_t)p.addend | (uintptr_t)p.mask_src) % 16 == 0;
+    if (g_replace_address && !g_tc_reg_epilogue && !p.serial_epilogue && p.bk == TC_BK && p.bn >= 64 && p.n_store == p.bn && (long)p.P * p.Q % TC_BM == 0 &&
+        (p.Q % 64 == 0 || 64 % p.Q == 0) && p.out_H % p.out_sh == 0 && p.out_W % p.out_sw == 0 && p.Cout % 4 == 0 && aligned) {
+        const int slot_bytes = (nops ? nops : 1) * 16384;
+        auto slots_beside = [&](int st) { return (int)((227L * 1024 - 1024 - (long)st * stage_bytes - 2 * st * 8) / (slot_bytes + 16)); };
+        while (slots_beside(stages) < 2 && stages > 4) stages--;  // short-K launches: the stages past 4 buy nothing
+        const int e = slots_beside(stages);
+        if (e >= 2) {
+            p.epi_slots = e < 4 ? e : 4;
+            p.epi_slot_bytes = slot_bytes;
+            const long ni = (long)p.G * p.B;
+            const int qbox = p.Q < 64 ? p.Q : 64;
+            if (int rc = encode_out_map(&p.ymap, p.y, ni, p.out_H, p.out_W, p.Cout, p.out_sh, p.out_sw, qbox)) return rc;
+            if (p.addend)
+                if (int rc = encode_out_map(&p.addmap, p.addend, ni, p.out_H, p.out_W, p.Cout, p.out_sh, p.out_sw, qbox)) return rc;
+            if (p.mask_src)
+                if (int rc = encode_out_map(&p.maskmap, p.mask_src, ni, p.out_H, p.out_W, p.Cout, p.out_sh, p.out_sw, qbox)) return rc;
+        }
+    }
+    p.stages = stages;
+    size_t smem = (size_t)stages * stage_bytes + 1024 /*align slack*/ + 2 * stages * 8 + (size_t)p.epi_slots * (p.epi_slot_bytes + 16);
     void (*kern)(TcParams) = p.bk == 32 ? tc_kernel_for<32>(p.bn) : tc_kernel_for<8>(p.bn);
     if (!kern) {
         set_error("conv_tc: no kernel for N tile %d / K chunk %d", p.bn, p.bk);

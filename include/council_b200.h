@@ -63,7 +63,9 @@ int cg_device_info(int* sm_count, int* cc_major, int* cc_minor);
  * on the previous tensor-core kernel, which transposes both operands in the MMA warps, for comparisons in one process (default:
  * the TMA-fed kernel that reads one operand from a channel-major copy), 1<<26 = the previous epilogue and tile walk of the
  * forward / data-gradient tensor-core kernel, which load the addend and mask one column group at a time and walk the parity
- * classes outermost, for comparisons in one process (same results).  Other bits are accepted and ignored.
+ * classes outermost, for comparisons in one process (same results), 1<<27 = every forward / data-gradient tensor-core launch on
+ * the register epilogue (default: the shared-memory epilogue, TMA-loaded addend and mask and TMA-stored results, wherever the
+ * tile geometry allows it), for comparisons in one process (same results).  Other bits are accepted and ignored.
  * The switches are per calling thread (like cg_last_error), not process-global.  Returns the previous mask. */
 int cg_set_tensor_core_mode(int mode);
 /* number of kernels launched by this library since load (bench.py reports it as gpu_launches) */

@@ -3,8 +3,9 @@ launches of the step, at their production shapes.
 
     python scripts/prof_conv_tc.py [iters]
 
-CUDA events over `iters` (default 20) launches after warm-up.  Every launch runs with the default epilogue and tile walk and with
-the previous ones (mode bit 26), alternating three times in one process; the best of the three is reported for each.  Prints ms per
+CUDA events over `iters` (default 20) launches after warm-up.  Every launch runs with the default epilogue and tile walk, with the
+register epilogue (mode bit 27) and with the previous epilogue and walk (mode bit 26), alternating three times in one process; the
+best of the three is reported for each.  Prints ms per
 launch, algorithmic TFLOP/s and its ratio to the TF32 cuBLAS rate measured in the same process (torch.matmul 8192^3, best of 10, as
 bench.py measures it), and the card it ran on with its power limit.  Epilogues as in the training step: the forward of the
 generator layers with the fused statistics, of the discriminator layers with bias and LeakyReLU; the data gradient of the
@@ -58,7 +59,7 @@ def timed(fn, iters):
     return e0.elapsed_time(e1) / iters
 
 
-MODES = [('default', 1), ('bit 26', 7 | (1 << 26))]
+MODES = [('default', 1), ('bit 27', 7 | (1 << 27)), ('bit 26', 7 | (1 << 26))]
 
 
 def main():
