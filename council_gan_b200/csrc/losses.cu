@@ -235,17 +235,36 @@ __global__ void __launch_bounds__(256) gen_loss_bwd_kernel(const cg_gen_loss_des
             const double msum = (double)scal[g * 6 + 3] / hp.numel;
             const double ltv = ((double)scal[g * 6 + 4] + (double)scal[g * 6 + 5]) / hp.numel;
             double tot = 0.0, ltot = 0.0, c01 = 0.0, csum = 0.0, ctv = 0.0;
+            const double* rg = hist_gan + (long)g * R;
+            const bool fm = hp.focus_on && hp.focus_matching;
+            // focus matching (:398-410, 433-445) runs before the GAN block: its ratios read the GAN history before this append
+            const double gan_before = fm ? ring_mean(rg, R, hp.head_gan, hp.hist_size, lane) : 1.0;
+            double w01m = 1.0, wtm = 1.0, l01_32 = 0.0, ltot_app = 0.0;
             if (hp.focus_on) {
-                if (hp.w01 != 0.0) { tot += hp.w01 * l01; c01 = hp.w01 / hp.numel; }            // trainer_council.py:392-415
-                if (hp.wtv != 0.0) { tot += hp.wtv * ltv; ctv = hp.wtv / hp.numel; }            // :425-431
+                if (hp.w01 != 0.0) {                                                             // trainer_council.py:392-415
+                    double s01 = 1.0;
+                    if (fm) {  // append the unscaled float32 term, then scale it in place by the float32 ratio
+                        l01_32 = (double)(float)l01;
+                        w01m = gan_before / ring_mean_after_append(hp.hist_focus01 + (long)g * R, R, hp.head_focus01, hp.hist_size, l01_32, lane);
+                        s01 = (double)(float)w01m;
+                    }
+                    tot += hp.w01 * l01 * s01;
+                    c01 = hp.w01 * s01 / hp.numel;
+                }
+                if (hp.wtv != 0.0) { tot += hp.wtv * ltv; ctv = hp.wtv / hp.numel; }            // :425-431 (never matched)
                 if (hp.wtot != 0.0) {                                                            // :418-422, :447-451
                     if (hp.small_abs) { ltot += fabs(msum); csum += hp.wtot * (double)((msum > 0.0) - (msum < 0.0)) / hp.numel; }
                     if (hp.small_square) { ltot += msum * msum; csum += hp.wtot * 2.0 * msum / hp.numel; }
+                    if (fm) {  // b2a appends a2b's scaled term (:441), a2b its own unscaled one (:435)
+                        ltot_app = hp.focus_src ? (double)hp.focus_src[g * 8 + 3] : (double)(float)ltot;
+                        wtm = gan_before / ring_mean_after_append(hp.hist_focus + (long)g * R, R, hp.head_focus, hp.hist_size, ltot_app, lane);
+                        ltot *= (double)(float)wtm;
+                        csum *= (double)(float)wtm;
+                    }
                     tot += hp.wtot * ltot;
                 }
             }
             double mean_gan;
-            const double* rg = hist_gan + (long)g * R;
             const double adv32 = (double)(float)adv;  // the history stores the float32 loss value (:520)
             if (hp.gan_on) {
                 mean_gan = hp.matching ? ring_mean_after_append(rg, R, hp.head_gan, hp.hist_size, adv32, lane)
@@ -275,11 +294,14 @@ __global__ void __launch_bounds__(256) gen_loss_bwd_kernel(const cg_gen_loss_des
                     total64[g] = t64;
                     total[g] = (float)t64;
                     float* o = pub + g * 8;
-                    o[0] = (float)tot; o[1] = (float)adv; o[2] = (float)l01; o[3] = (float)ltot; o[4] = (float)ltv;
+                    o[0] = (float)tot; o[1] = (float)adv; o[2] = (float)(l01 * (double)(float)w01m); o[3] = (float)ltot; o[4] = (float)ltv;
                     o[5] = (float)closs; o[6] = (float)w; o[7] = (float)cl;
                     if (hp.gan_on && hp.matching) hist_gan[(long)g * R + (hp.head_gan + hp.hist_size) % R] = adv32;
                     if (hp.council_on && hp.matching)
                         hist_council[(long)g * R + (hp.head_council + hp.hist_size) % R] = (double)(float)cl;
+                    if (fm && hp.w01 != 0.0) hp.hist_focus01[(long)g * R + (hp.head_focus01 + hp.hist_size) % R] = l01_32;
+                    if (fm && hp.wtot != 0.0) hp.hist_focus[(long)g * R + (hp.head_focus + hp.hist_size) % R] = ltot_app;
+                    if (hp.focus_w) { hp.focus_w[g * 2] = (float)w01m; hp.focus_w[g * 2 + 1] = (float)wtm; }
                 }
             }
         }
@@ -784,6 +806,12 @@ extern "C" int cg_gen_loss_bwd(const cg_gen_loss_desc* d, const cg_gen_loss_hp* 
     CG_REQUIRE(hp && hp->world >= 1 && hp->hist_size >= 1 && hp->numel > 0, "gen_loss_bwd: bad hyper-parameters");
     CG_REQUIRE(ws_bytes >= 16 + CG_LOSS_MAX_G * 8, "gen_loss_bwd: workspace too small");
     CG_REQUIRE(!d_mask || d->mask, "gen_loss_bwd: d_mask without mask");
+    if (hp->focus_matching && hp->focus_on) {
+        CG_REQUIRE((hp->w01 == 0.0 || hp->hist_focus01) && (hp->wtot == 0.0 || hp->hist_focus),
+                   "gen_loss_bwd: focus matching without its history rings");
+        CG_REQUIRE(hp->head_focus >= 0 && hp->head_focus <= hp->hist_size && hp->head_focus01 >= 0 && hp->head_focus01 <= hp->hist_size,
+                   "gen_loss_bwd: focus history heads out of range");
+    }
     for (int m = 0; m < d->n_cl; m++) CG_REQUIRE(d->cl_dout[m] && d->cl_out[m], "gen_loss_bwd: council map %d without buffers", m);
     int map_blocks = d->n_cl * d->G;
     long total_px = d_mask ? (long)d->G * d->B * d->H * d->W : 0;

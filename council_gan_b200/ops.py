@@ -45,7 +45,9 @@ class GenLossDesc(C.Structure):  # cg_gen_loss_desc
 class GenLossHp(C.Structure):  # cg_gen_loss_hp
     _fields_ = [(n, C.c_int32) for n in ('world', 'hist_size', 'head_gan', 'head_council', 'gan_on', 'council_on', 'focus_on',
                                          'matching', 'small_abs', 'small_square')] + \
-               [(n, C.c_double) for n in ('gan_w', 'council_w', 'w01', 'wtot', 'wtv', 'numel')]
+               [(n, C.c_double) for n in ('gan_w', 'council_w', 'w01', 'wtot', 'wtv', 'numel')] + \
+               [(n, C.c_int32) for n in ('focus_matching', 'head_focus', 'head_focus01', '_pad')] + \
+               [(n, C.c_void_p) for n in ('hist_focus', 'hist_focus01', 'focus_src', 'focus_w')]
 
 
 _fp = C.c_void_p
@@ -637,17 +639,26 @@ class CudaOps:
         self._ck(self.lib.cg_gen_loss_fwd(C.byref(d), _p(scal), _p(ws), ws.numel(), self._stream()), 'cg_gen_loss_fwd')
         return adv_douts
 
-    def gen_loss_bwd(self, cl_outs, mask, center, eps, scal, hp, hist_gan, hist_council, total, accumulate, pub, want_dmask):
+    def gen_loss_bwd(self, cl_outs, mask, center, eps, scal, hp, hist_gan, hist_council, total, accumulate, pub, want_dmask, *,
+                     hist_focus=None, hist_focus01=None, focus_src=None, focus_w=None):
         """Pass 2: loss assembly, history matching and publication on the device + council-map / mask gradients, ONE launch.
-        hp: dict with the cg_gen_loss_hp fields.  Returns (cl_douts, d_mask or None)."""
-        self._chk(scal, mask, total, pub, *cl_outs)
+        hp: dict with the cg_gen_loss_hp scalar fields.  Returns (cl_douts, d_mask or None).
+        Focus matching (hp['focus_matching'], heads hp['head_focus'] / hp['head_focus01']): hist_focus / hist_focus01 are the float64
+        rings [G, hist+1] of the mask-total and zero-one terms; focus_src the a2b call's pub [G, 8] when this is the b2a call;
+        focus_w (optional, [G, 2]) receives the two ratios of every member."""
+        self._chk(scal, mask, total, pub, focus_src, focus_w, *cl_outs)
         assert hist_gan.dtype == torch.float64 and hist_council.dtype == torch.float64
+        for r in (hist_focus, hist_focus01):
+            assert r is None or (r.dtype == torch.float64 and r.is_contiguous() and tuple(r.shape) == tuple(hist_gan.shape))
         cl_douts = [torch.empty_like(o) for o in cl_outs]
         d = self._gen_desc([], cl_outs, mask, center, eps, 0.0, None, cl_douts)
         d.G = total.shape[0]
+        assert focus_src is None or focus_src.numel() == d.G * 8
+        assert focus_w is None or focus_w.numel() == d.G * 2
         h = GenLossHp()
         for k, v in hp.items():
             setattr(h, k, v)
+        h.hist_focus, h.hist_focus01, h.focus_src, h.focus_w = _p(hist_focus), _p(hist_focus01), _p(focus_src), _p(focus_w)
         d_mask = torch.empty_like(mask) if want_dmask else None
         ws = self._loss_scratch(d.G, d.B, d.H, d.W)
         self._ck(self.lib.cg_gen_loss_bwd(C.byref(d), C.byref(h), _p(scal), hist_gan.data_ptr(), hist_council.data_ptr(), _p(total),

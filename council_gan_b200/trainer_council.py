@@ -65,6 +65,14 @@ What is different underneath (GPU-first, see DESIGN.md):
     scalar all-reduce) and its gradient; the VGG data gradient runs before the per-direction backward, and its d(x_fake) joins d_x.
     ``loss_gen_vgg_{a,b}_s`` are published through the reconstruction terms' finalize launch.  The network is not one of the
     trainer's networks: no optimiser state, checkpoint or all-reduce.  With vgg_w 0 (the shipped configs) nothing of it runs.
+  * do_w_loss_matching_focus (:398-410, 433-445, ``focus_loss.do_w_loss_matching_focus``): while the focus gate is open, gen_update's
+    pass 2 scales the zero-one term (mask_zero_or_one_w != 0) and the mask-total term of each member by mean(its GAN history before
+    this update's append) / mean(its own focus history after appending the unscaled term), the ratio rounded to float32.  The
+    b2a mask-total history appends a2b's SCALED term (:441), read from a2b's published values on the device.  The two float64 rings
+    per direction live on the device like the GAN / council ones; ``los_hist_focus{,_zero_one}_{a2b,b2a}_s`` read them back and
+    ``w_match_focus{,_zero_one}_{a2b,b2a}_conf`` keep the last member's ratios.  No launch is added.  A focus weight with
+    mask_total_w 0 or without do_a2b raises NotImplementedError (the reference fails there).  Off (the shipped configs), or with
+    both focus weights 0, nothing of it runs.
   * pad_type: reflect (networks.py:463-520, ``gen.pad_type`` / ``dis.pad_type``; every shipped config documents zero/reflect): each
     Conv2dBlock with a pad reads a reflect-padded copy of its input (cg_reflect_pad) through a convolution with pad 0, and the weight
     gradient reads that copy, kept instead of the input.  The data gradient runs at the padded shape, and cg_reflect_pad_bwd folds the
@@ -72,8 +80,8 @@ What is different underneath (GPU-first, see DESIGN.md):
     the same pass instead of folding the upsample into the convolution.  The AvgPool pyramid, the MLP, the 1x1 layers and the VGG keep
     zero padding; parameter names and checkpoints do not change.  Other pad types fail the networks' assertion.  With zero (the
     shipped configs) nothing of it runs.
-Paths outside the live configuration space of the reference's three configs (recon_x_cyc loss, nsgan/RaHinge, do_my_style,
-do_w_loss_matching_focus) raise NotImplementedError.
+Paths outside the live configuration space of the reference's three configs (recon_x_cyc loss, nsgan/RaHinge, do_my_style)
+raise NotImplementedError.
 """
 from __future__ import annotations
 
@@ -170,7 +178,9 @@ class Council_Trainer(nn.Module):
         self._check_supported(hp)
         self._dirs = [d for d in _DIRS if hp['do_' + d]]
         N, hist = self.council_size, self.los_matching_hist_size_conf
-        for d in self._dirs:  # :70-92; the gan / council histories live on the device (see _rings), these two are never updated
+        focus_match = bool(self.do_w_loss_matching_focus)
+        for d in self._dirs if not focus_match else ():  # :70-92; the gan / council histories live on the device (see _rings);
+            # without focus matching these two are never updated
             setattr(self, 'los_hist_focus_%s_s' % d, [deque(np.ones(hist)) for _ in range(N)])
             setattr(self, 'los_hist_focus_zero_one_%s_s' % d, [deque(np.ones(hist)) for _ in range(N)])
         self.do_council_loss = None
@@ -185,6 +195,11 @@ class Council_Trainer(nn.Module):
         rings = {d: {'gan': torch.ones(N, hist + 1, dtype=torch.float64).to(_ops.device),
                      'council': torch.ones(N, hist + 1, dtype=torch.float64).to(_ops.device),
                      'head_gan': 0, 'head_council': 0} for d in self._dirs}
+        if focus_match:  # the focus histories (:398-445) likewise, exported by los_hist_focus{,_zero_one}_{a2b,b2a}_s
+            for d in self._dirs:
+                for kind in ('focus', 'focus_zero_one'):
+                    rings[d][kind] = torch.ones(N, hist + 1, dtype=torch.float64).to(_ops.device)
+                    rings[d]['head_' + kind] = 0
         object.__setattr__(self, '_rings', rings)
         dist = _dist()
         self.world = dist.get_world_size() if dist else 1
@@ -235,10 +250,11 @@ class Council_Trainer(nn.Module):
 
     def __getattr__(self, name):
         # los_hist_gan_a2b_s etc. (trainer_council.py:81-92): lists of deques, read back from the device rings on demand
-        if name.startswith('los_hist_gan_') or name.startswith('los_hist_council_'):
-            kind, d = ('gan', name[13:16]) if name.startswith('los_hist_gan_') else ('council', name[17:20])
+        kind = next((k for k in ('gan', 'council', 'focus_zero_one', 'focus') if name.startswith('los_hist_%s_' % k)), None)
+        if kind is not None:
+            d = name[len('los_hist_%s_' % kind):][:3]
             rings = self.__dict__.get('_rings', {})
-            if d in rings and name.endswith('_s'):
+            if d in rings and kind in rings[d] and name == 'los_hist_%s_%s_s' % (kind, d):
                 r = rings[d]
                 R = r[kind].shape[1]
                 host = r[kind].detach().cpu().numpy()
@@ -281,8 +297,13 @@ class Council_Trainer(nn.Module):
                                       'needs do_a2b and do_b2a (with one direction the reference fails with an AttributeError)')
         if hp['dis']['gan_type'] != 'lsgan':
             assert 0, "Unsupported GAN type: {}".format(hp['dis']['gan_type'])
-        if hp['focus_loss'].get('do_w_loss_matching_focus'):
-            raise NotImplementedError('do_w_loss_matching_focus is not on the accelerated path')
+        if hp['focus_loss'].get('do_w_loss_matching_focus') and (hp['mask_zero_or_one_w'] != 0 or hp['mask_total_w'] != 0):
+            if hp['mask_total_w'] == 0:
+                raise NotImplementedError('do_w_loss_matching_focus matches the mask-total term whenever the focus gate is open, so it '
+                                          'needs mask_total_w != 0 (with mask_total_w 0 the reference fails with an AttributeError)')
+            if not hp['do_a2b']:
+                raise NotImplementedError('do_w_loss_matching_focus fills the b2a mask-total history from the a2b term, so it needs '
+                                          'do_a2b (with b2a alone the reference fails with an IndexError)')
         if not (hp['do_a2b'] or hp['do_b2a']):
             raise ValueError('at least one of do_a2b / do_b2a must be set')
 
@@ -717,6 +738,9 @@ class Council_Trainer(nn.Module):
         if ca_on:
             ca_pub = ops.empty(nd, N)
         matching = bool(self.do_w_loss_matching)
+        focus_match = focus_on and bool(self.do_w_loss_matching_focus)
+        if focus_match:
+            focus_w = ops.empty(nd, N, 2)  # per direction and member: the zero-one and mask-total ratios
         data_parallel = self.world > 1
         recon_x_on = hp['recon_x_w'] != 0
 
@@ -735,9 +759,18 @@ class Council_Trainer(nn.Module):
                    'small_square': int(bool(fl['mask_small_use_square'])), 'gan_w': float(hp['gan_w']),
                    'council_w': float(hp['council_w']), 'w01': float(hp['mask_zero_or_one_w']), 'wtot': float(hp['mask_total_w']),
                    'wtv': float(hp['mask_tv_w']), 'numel': float(rec['B'] * self.world * 3 * rec['H'] * rec['W'])}
+            focus_kw = {}
+            if focus_match:  # :398-410, 433-445; b2a's mask-total history appends a2b's scaled term (:441), pub[0][:, 3]
+                hpd.update(focus_matching=1, head_focus=ring['head_focus'], head_focus01=ring['head_focus_zero_one'])
+                focus_kw = dict(hist_focus=ring['focus'], hist_focus01=ring['focus_zero_one'], focus_w=focus_w[di],
+                                focus_src=pub[self._dirs.index('a2b')] if d == 'b2a' else None)
             d_cl, d_mask = ops.gen_loss_bwd(rec['disc_outs'], rec['mask'] if focus_on else None, center, eps, scal[di], hpd,
-                                            ring['gan'], ring['council'], total, di > 0, pub[di], focus_on)
+                                            ring['gan'], ring['council'], total, di > 0, pub[di], focus_on, **focus_kw)
             R = self.los_matching_hist_size_conf + 1
+            if focus_match and hp['mask_zero_or_one_w'] != 0:
+                ring['head_focus_zero_one'] = (ring['head_focus_zero_one'] + 1) % R
+            if focus_match:  # the mask-total term is matched whenever the gate is open (mask_total_w != 0, _check_supported)
+                ring['head_focus'] = (ring['head_focus'] + 1) % R
             if gan_on and matching:  # :518-524 append + popleft
                 ring['head_gan'] = (ring['head_gan'] + 1) % R
             if council_on and matching:  # :576-586
@@ -803,6 +836,10 @@ class Council_Trainer(nn.Module):
                 setattr(self, 'council_loss_%s_s' % ab, col(5) if council_on or ca_on else [0] * N)
                 if council_on and matching:
                     setattr(self, 'w_match_%s_conf' % d, pub[di, N - 1, 6])  # the reference keeps the last member's ratio (:583)
+                if focus_match:  # likewise for the focus ratios (:402, 408, 437, 443)
+                    if hp['mask_zero_or_one_w'] != 0:
+                        setattr(self, 'w_match_focus_zero_one_%s_conf' % d, focus_w[di, N - 1, 0])
+                    setattr(self, 'w_match_focus_%s_conf' % d, focus_w[di, N - 1, 1])
             else:
                 setattr(self, 'loss_gen_adv_%s_s' % d, [0] * N if gan_on else [])
                 setattr(self, 'loss_gen_mask_zero_one_%s_s' % ab, [])

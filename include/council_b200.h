@@ -223,6 +223,15 @@ typedef struct {
     int32_t gan_on, council_on, focus_on, matching, small_abs, small_square;
     double gan_w, council_w, w01, wtot, wtv;  /* loss weights (0 = term off)                                        */
     double numel;                             /* mask.numel() of the GLOBAL minibatch                               */
+    /* do_w_loss_matching_focus (trainer_council.py:398-410, 433-445); all zero = off.  While focus_on, each focus term is
+     * scaled by mean(GAN history BEFORE this call's append) / mean(its own history after the append), the ratio rounded to
+     * float32: the zero-one term (w01 != 0) through hist_focus01, the mask-total term (wtot != 0) through hist_focus.      */
+    int32_t focus_matching, head_focus, head_focus01, _pad;
+    double* hist_focus;                       /* double[G][hist_size+1]: appends the unscaled float32 mask-total term  */
+    double* hist_focus01;                     /* double[G][hist_size+1]: appends the unscaled float32 zero-one term    */
+    const float* focus_src;                   /* NULL, or the pub[G][8] of the a2b call: the b2a history then appends   *
+                                               * its column 3, a2b's SCALED mask-total term (:441)                      */
+    float* focus_w;                           /* NULL, or [G][2] = { zero-one ratio, mask-total ratio } (1: not scaled)  */
 } cg_gen_loss_hp;
 /* pass 1: scal[G][6] = { sum_scales mean (D(x)-1)^2, sum_scales mean (DC(x)-1)^2, sum 1/(|m-c|+eps), sum m,
  * sum |dh m|, sum |dw m| } for this rank, and the gradient of the adversarial maps (calc_gen_loss networks.py:84-90,188-194;
@@ -232,7 +241,9 @@ int cg_gen_loss_fwd(const cg_gen_loss_desc* d, float* scal, void* ws, size_t ws_
  * 559-634), appends to the loss histories and derives w_match (:518-524,576-586), publishes
  * pub[G][8] = { total of this direction, adv, zero_one, mask_total, TV, council loss, w_match, raw council },
  * total[g] (+)= direction total, and writes the council-map and mask gradients.  The caller advances head_gan /
- * head_council by one after a call that appended (gan_on && matching / council_on && matching). */
+ * head_council by one after a call that appended (gan_on && matching / council_on && matching), and head_focus01 /
+ * head_focus after a call that appended to those (focus_on && focus_matching, with w01 != 0 / wtot != 0).  With
+ * focus_matching, zero_one and mask_total in pub are the scaled values. */
 int cg_gen_loss_bwd(const cg_gen_loss_desc* d, const cg_gen_loss_hp* hp, const float* scal, double* hist_gan,
                     double* hist_council, float* total, int accumulate, float* pub, float* d_mask, void* ws,
                     size_t ws_bytes, void* stream);
