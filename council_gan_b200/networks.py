@@ -104,9 +104,10 @@ class LayerSpec:
         self.linear = linear
         self.wname = key + '.weight'
         self.bname = key + '.bias'
+        self.vecs = []  # names of per-channel [cout] parameters stored before the weight (a layer norm's gamma / beta)
 
     def entries(self):
-        return [(self.wname, (self.cout, self.k, self.k, self.cin_p)), (self.bname, (self.cout,))]
+        return [(n, (self.cout,)) for n in self.vecs] + [(self.wname, (self.cout, self.k, self.k, self.cin_p)), (self.bname, (self.cout,))]
 
     # reference <-> kernel layout
     def export_weight(self, w):  # w: [Cout,KH,KW,Cin_p] one member
@@ -192,6 +193,8 @@ class _StackedNet:
             b = self._bank_of(spec.wname)
             sd[spec.wname] = spec.export_weight(b.p(spec.wname)[i])
             sd[spec.bname] = b.p(spec.bname)[i].clone()
+            for n in spec.vecs:
+                sd[n] = b.p(n)[i].clone()
         for k, v in self.extra_state().items():
             sd[k] = v.clone()
         # reference key order (state_dict of the nn.Module tree)
@@ -211,6 +214,9 @@ class _StackedNet:
                 spec.import_weight(b.p(spec.wname)[i], sd[spec.wname])
             if spec.bname in sd:
                 b.p(spec.bname)[i].copy_(sd[spec.bname].detach().to('cpu', b.data.dtype).reshape(-1))
+            for n in spec.vecs:
+                if n in sd:
+                    b.p(n)[i].copy_(sd[n].detach().to('cpu', b.data.dtype).reshape(-1))
         self.params_changed()
 
     def params_changed(self):
@@ -671,12 +677,25 @@ class CouncilGen(_StackedNet):
 # discriminators
 # ------------------------------------------------------------------------------------------------------
 class CouncilDis(_StackedNet):
-    """MsImageDis (council=False) / MsImageDisCouncil (council=True), all members stacked."""
+    """MsImageDis (council=False) / MsImageDisCouncil (council=True), all members stacked.
+
+    dis.norm (networks.py:40-44, 137-143): layers 1 .. n_layer-1 of every scale normalise between the convolution and the LeakyReLU.
+      * 'in'  -- nn.InstanceNorm2d (no parameters): the convolution's epilogue gives the statistics (cg_conv_fwd_stats), then one
+                 normalise + LeakyReLU pass.  The conv bias is removed again by the mean subtraction: it is never added and its
+                 gradient is exactly 0 (as the generators' dead biases).
+      * 'ln'  -- LayerNorm (networks.py:659-686): the convolution with its (live) bias, the per-sample statistics over C*H*W with the
+                 unbiased std (cg_ln_stats), then (y - mean) / (std + eps) * gamma + beta and the LeakyReLU (cg_ln_act_fwd).  gamma /
+                 beta are bank entries 'cnns.<s>.<i>.norm.{gamma,beta}', stored before the block's conv weight and bias as the
+                 reference's parameters() lists them.
+    """
+
+    NORMS = ('none', 'in', 'ln')
 
     def __init__(self, ops, hp, G, input_dim=3, council=False):
         dp = hp['dis']
         assert dp['gan_type'] == 'lsgan', 'only the LSGAN objective is on the accelerated path'
-        assert dp['norm'] == 'none' and dp['activ'] == 'lrelu'
+        assert dp['norm'] in self.NORMS and dp['activ'] == 'lrelu'
+        self.norm = dp['norm']
         self.reflect = _pad_type(dp['pad_type'])
         assert input_dim == 3
         self.ops, self.hp, self.G, self.council = ops, hp, G, council
@@ -689,7 +708,10 @@ class CouncilDis(_StackedNet):
             else:        # networks.py:40: 4x4 stride 2
                 layers = [LayerSpec('cnns.%d.0.conv' % sc, d, input_dim, 4, 2, 1, lanes=[0, 1, 2])]
             for i in range(self.n_layer - 1):
-                layers.append(LayerSpec('cnns.%d.%d.conv' % (sc, i + 1), 2 * d, d, 4, 2, 1))
+                s = LayerSpec('cnns.%d.%d.conv' % (sc, i + 1), 2 * d, d, 4, 2, 1)
+                if self.norm == 'ln':
+                    s.vecs = ['cnns.%d.%d.norm.gamma' % (sc, i + 1), 'cnns.%d.%d.norm.beta' % (sc, i + 1)]
+                layers.append(s)
                 d *= 2
             n = self.n_layer
             tail = []
@@ -700,6 +722,9 @@ class CouncilDis(_StackedNet):
             self.scales.append((layers, tail))
         self.specs = [s for layers, tail in self.scales for s in layers + tail]
         self.bank = ParamBank(ops, G, [e for s in self.specs for e in s.entries()])
+        # the normalised layers, and under 'in' their dead conv biases (their gradient stays exactly 0)
+        self.normed = set(s.key for layers, _ in self.scales for s in layers[1:]) if self.norm != 'none' else set()
+        self.dead_bias = set(s.bname for s in self.specs if s.key in self.normed) if self.norm == 'in' else set()
 
     def _specs(self):
         return self.specs
@@ -712,7 +737,38 @@ class CouncilDis(_StackedNet):
         return ParamBank(self.ops, self.G, [e for s in self.specs for e in s.entries()], trainable=False)
 
     def reference_key_order(self):
-        return [k for s in self.specs for k in (s.wname, s.bname)]
+        return [k for s in self.specs for k in s.vecs + [s.wname, s.bname]]
+
+    def _conv_norm(self, h, s, bank, pad):
+        """Conv2dBlock.forward of a normalised layer: -> (LeakyReLU output, what _conv_norm_bwd needs)"""
+        ops = self.ops
+        w = bank.p(s.wname)
+        G, B = w.shape[0], h.shape[1]
+        ho = (h.shape[2] + 2 * pad - s.k) // s.stride + 1
+        wo = (h.shape[3] + 2 * pad - s.k) // s.stride + 1
+        if self.norm == 'in':
+            if ho * wo == 1:  # nn.InstanceNorm2d in training mode (F.instance_norm's check)
+                raise ValueError('Expected more than 1 spatial element when training, got input size torch.Size([%d, %d, 1, 1])'
+                                 % (B, s.cout))
+            y, mean, rstd = ops.conv_fwd_stats(h, w, s.stride, pad)
+            return ops.norm_act_fwd(y, mean, rstd, act=ACT_LRELU), (y, mean, rstd)
+        y = ops.conv_fwd(h, w, bank.p(s.bname), s.stride, pad)
+        mean, std = ops.ln_stats(y)
+        gamma, beta = bank.p(s.vecs[0]), bank.p(s.vecs[1])
+        return ops.ln_act_fwd(y, mean, std, gamma, beta, act=ACT_LRELU), (y, mean, std)
+
+    def _conv_norm_bwd(self, d, s, rec, bank, want_wgrad):
+        """d(LeakyReLU output) of a normalised layer -> d(conv output); under 'ln' with want_wgrad also d gamma / d beta"""
+        ops = self.ops
+        y, mean, st = rec
+        if self.norm == 'in':
+            return ops.norm_act_bwd(d, y, mean, st, act=ACT_LRELU)
+        gamma, beta = bank.p(s.vecs[0]), bank.p(s.vecs[1])
+        if want_wgrad:
+            dgamma, dbeta = bank.g(s.vecs[0]), bank.g(s.vecs[1])
+        else:  # the data gradient alone (gen_update): the parameter gradients go to scratch
+            dgamma, dbeta = ops.empty(*gamma.shape), ops.empty(*beta.shape)
+        return ops.ln_act_bwd(d, y, mean, st, gamma, beta, dgamma, dbeta, act=ACT_LRELU)
 
     def forward(self, x, saved=None, bank=None):
         """x [G,Bt,H,W,4|8] -> list over scales of patch outputs [G,Bt,h,w,1].  bank: parameters laid out like self.bank (None:
@@ -722,17 +778,21 @@ class CouncilDis(_StackedNet):
         for sc, (layers, tail) in enumerate(self.scales):
             h = x
             acts = []  # the input of each layer (padded under reflect), then the output
-            for s in layers:
+            norms = {}  # layer index -> the record of its normalisation
+            for li, s in enumerate(layers):
                 h, pad = _padded(ops, h, s, self.reflect)
                 acts.append(h)
-                h = ops.conv_fwd(h, bank.p(s.wname), bank.p(s.bname), s.stride, pad, act=ACT_LRELU, slope=0.2)
+                if s.key in self.normed:
+                    h, norms[li] = self._conv_norm(h, s, bank, pad)
+                else:
+                    h = ops.conv_fwd(h, bank.p(s.wname), bank.p(s.bname), s.stride, pad, act=ACT_LRELU, slope=0.2)
             for s in tail:
                 acts.append(h)
                 h = ops.conv_fwd(h, bank.p(s.wname), bank.p(s.bname), 1, 0)
             acts.append(h)
             outs.append(h)
             if saved is not None:
-                saved.append(acts)
+                saved.append((acts, norms))
             if sc + 1 < self.num_scales:
                 x = ops.avgpool_fwd(x)
         return outs
@@ -744,7 +804,7 @@ class CouncilDis(_StackedNet):
         ops, bank = self.ops, self.bank if bank is None else bank
         dx_scales = []
         for sc, (layers, tail) in enumerate(self.scales):
-            acts = saved[sc]
+            acts, norms = saved[sc]
             d = d_outs[sc]
             allspecs = layers + tail
             nl = len(layers)
@@ -753,13 +813,15 @@ class CouncilDis(_StackedNet):
                 a_in = acts[li]
                 reflect = self.reflect and s.pad > 0
                 pad = 0 if reflect else s.pad
+                if li in norms:  # d arrives as d(LeakyReLU output), ungated: through the LeakyReLU and the norm to d(conv output)
+                    d = self._conv_norm_bwd(d, s, norms[li], bank, want_wgrad)
                 if want_wgrad:
-                    ops.conv_wgrad(a_in, d, bank.g(s.wname), bank.g(s.bname), s.stride, pad)
+                    ops.conv_wgrad(a_in, d, bank.g(s.wname), None if s.bname in self.dead_bias else bank.g(s.bname), s.stride, pad)
                 if li == 0 and not want_dx:
                     break
                 # a_in is the lrelu OUTPUT of layer li-1 when that layer is one of `layers` (padded under reflect: the gate read from
-                # it gates every copy of a pixel alike)
-                masked = 1 <= li <= nl
+                # it gates every copy of a pixel alike); a normalised layer li-1 applies its LeakyReLU gate in its own backward
+                masked = 1 <= li <= nl and (li - 1) not in norms
                 d = ops.conv_dgrad(d, bank.p(s.wname), a_in.shape, s.stride, pad,
                                    mask_src=a_in if masked else None, mask_slope=0.2)
                 if reflect:

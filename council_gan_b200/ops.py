@@ -66,6 +66,10 @@ _SIGS = {
     'cg_in_stats': (C.c_int, [_fp, _fp, _fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, _fp, C.c_size_t, _fp]),
     'cg_norm_act_fwd': (C.c_int, [_fp, _fp, _fp, _fp, C.c_int, C.c_int, _fp, _fp] + [C.c_int] * 7 + [_fp]),
     'cg_norm_act_bwd': (C.c_int, [_fp, _fp, _fp, _fp, _fp, C.c_int, C.c_int, _fp, _fp] + [C.c_int] * 7 + [_fp, C.c_size_t, _fp]),
+    'cg_ln_workspace_bytes': (C.c_size_t, [C.c_int] * 4),
+    'cg_ln_stats': (C.c_int, [_fp, _fp, _fp] + [C.c_int] * 4 + [_fp, C.c_size_t, _fp]),
+    'cg_ln_act_fwd': (C.c_int, [_fp] * 5 + [C.c_float, _fp] + [C.c_int] * 6 + [_fp]),
+    'cg_ln_act_bwd': (C.c_int, [_fp] * 6 + [C.c_float] + [_fp] * 3 + [C.c_int] * 6 + [_fp, C.c_size_t, _fp]),
     'cg_upsample2x_bwd': (C.c_int, [_fp, _fp, C.c_int, C.c_int, C.c_int, C.c_int, _fp]),
     'cg_mask_head_fwd': (C.c_int, [_fp, _fp, _fp, _fp, C.c_int, C.c_int, C.c_int, _fp]),
     'cg_head_fused': (C.c_int, [_fp, _fp, _fp, _fp, C.c_int, C.c_int] + [_fp] * 9 + [C.c_int] * 3 + [_fp]),
@@ -356,6 +360,41 @@ class CudaOps:
                         lambda: self._ck(self.lib.cg_norm_act_bwd(_p(dz), _p(y), _p(mean), _p(rstd), _p(adain), P, off, _p(dy), _p(d_adain),
                                                                   G, B, H, W, Cc, act, int(bool(ups)), _p(ws), ws.numel(), self._stream()),
                                          'cg_norm_act_bwd'))
+        return dy
+
+    # -- layer norm (the discriminators' dis.norm ln) -------------------------------------------------
+    def ln_stats(self, y):
+        """-> (mean, std) [G,B]: each sample's mean and unbiased std over H*W*C"""
+        self._chk(y)
+        G, B, H, W, Cc = y.shape
+        mean, std = self.empty(G, B), self.empty(G, B)
+        ws = self._ws_for(self.lib.cg_ln_workspace_bytes(G, B, H * W, Cc))
+        self._timed_raw('hbm:ln_stats G%d B%d %dx%d C%d' % (G, B, H, W, Cc), 4.0 * y.numel(),
+                        lambda: self._ck(self.lib.cg_ln_stats(_p(y), _p(mean), _p(std), G, B, H * W, Cc, _p(ws), ws.numel(),
+                                                              self._stream()), 'cg_ln_stats'))
+        return mean, std
+
+    def ln_act_fwd(self, y, mean, std, gamma, beta, act=ACT_LRELU, eps=1e-5):
+        """act((y - mean) / (std + eps) * gamma + beta); gamma, beta [G,C]"""
+        self._chk(y, mean, std, gamma, beta)
+        G, B, H, W, Cc = y.shape
+        z = self.empty(G, B, H, W, Cc)
+        self._timed_raw('hbm:ln_act_fwd G%d B%d %dx%d C%d' % (G, B, H, W, Cc), 8.0 * y.numel(),
+                        lambda: self._ck(self.lib.cg_ln_act_fwd(_p(y), _p(mean), _p(std), _p(gamma), _p(beta), eps, _p(z), G, B, H, W, Cc,
+                                                                act, self._stream()), 'cg_ln_act_fwd'))
+        return z
+
+    def ln_act_bwd(self, dz, y, mean, std, gamma, beta, dgamma, dbeta, act=ACT_LRELU, eps=1e-5):
+        """-> d(y); dgamma, dbeta [G,C] are OUTPUT views (overwritten with the sums over each member's samples)"""
+        self._chk(dz, y, mean, std, gamma, beta, dgamma, dbeta)
+        G, B, H, W, Cc = y.shape
+        dy = self.empty(G, B, H, W, Cc)
+        ws = self._ws_for(self.lib.cg_ln_workspace_bytes(G, B, H * W, Cc))
+        # two passes over (y, dz) -- the reduction, then the apply -- and one write of dy
+        self._timed_raw('hbm:ln_act_bwd G%d B%d %dx%d C%d' % (G, B, H, W, Cc), 20.0 * y.numel(),
+                        lambda: self._ck(self.lib.cg_ln_act_bwd(_p(dz), _p(y), _p(mean), _p(std), _p(gamma), _p(beta), eps, _p(dy),
+                                                                _p(dgamma), _p(dbeta), G, B, H, W, Cc, act, _p(ws), ws.numel(),
+                                                                self._stream()), 'cg_ln_act_bwd'))
         return dy
 
     def upsample2x_bwd(self, d_up):

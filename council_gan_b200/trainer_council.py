@@ -80,6 +80,10 @@ What is different underneath (GPU-first, see DESIGN.md):
     the same pass instead of folding the upsample into the convolution.  The AvgPool pyramid, the MLP, the 1x1 layers and the VGG keep
     zero padding; parameter names and checkpoints do not change.  Other pad types fail the networks' assertion.  With zero (the
     shipped configs) nothing of it runs.
+  * dis.norm: in / ln (networks.py:40-44, 137-143, 659-686): both discriminator families normalise layers 1 .. n_layer-1 between
+    the convolution and the LeakyReLU (CouncilDis).  'ln' adds each block's LayerNorm gamma / beta to the discriminator banks, the
+    checkpoints and optimizer_<i>.pt in the reference's parameter order; gamma starts U(0,1), beta 0.  'bn' and 'sn' raise
+    NotImplementedError; other values fail the networks' assertion.  With none (the shipped configs) nothing of it runs.
 Paths outside the live configuration space of the reference's three configs (recon_x_cyc loss, nsgan/RaHinge, do_my_style)
 raise NotImplementedError.
 """
@@ -99,6 +103,14 @@ from .networks import IMG_C, CouncilDis, CouncilGen, Vgg16
 from .utils import get_model_list
 
 _DIRS = ('a2b', 'b2a')
+
+
+class _VecEntry:
+    """A per-channel parameter that is not a layer's bias (a layer norm's gamma / beta) in the optimiser's parameter list"""
+
+    def __init__(self, name):
+        self.key = self.bname = name
+        self.wname = None
 
 
 def _dist():
@@ -304,13 +316,18 @@ class Council_Trainer(nn.Module):
             if not hp['do_a2b']:
                 raise NotImplementedError('do_w_loss_matching_focus fills the b2a mask-total history from the a2b term, so it needs '
                                           'do_a2b (with b2a alone the reference fails with an IndexError)')
+        if hp['dis']['norm'] in ('bn', 'sn'):
+            raise NotImplementedError('dis.norm %s is not on the accelerated training path (in, ln and none are): batch norm takes '
+                                      'statistics across the batch of each forward and would need them synchronised across ranks; '
+                                      'spectral norm is not a documented option' % hp['dis']['norm'])
         if not (hp['do_a2b'] or hp['do_b2a']):
             raise ValueError('at least one of do_a2b / do_b2a must be set')
 
     def _init_weights(self, init_type):
         """weights_init (utils.py:402-422): kaiming fan_in normal (or N(0,0.02)) for generators, N(0,0.02) for
-        discriminators, zero biases.  Drawn from the torch CPU generator; the stream is not the reference's
-        (module construction order differs) -- parity tests load explicit state_dicts instead."""
+        discriminators, zero biases.  A layer norm's gamma is U(0,1) and its beta 0, as LayerNorm.__init__ draws them
+        (networks.py:666-667; weights_init touches Conv and Linear modules only).  Drawn from the torch CPU generator; the
+        stream is not the reference's (module construction order differs) -- parity tests load explicit state_dicts instead."""
         for name, net in self._nets.items():
             kind = init_type if name.startswith('gen_') else 'gaussian'
             if kind not in ('gaussian', 'kaiming', 'default'):
@@ -323,6 +340,8 @@ class Council_Trainer(nn.Module):
                 ref = torch.randn(net.G, spec.cout, spec.cin, spec.k, spec.k) * std
                 for i in range(net.G):
                     spec.import_weight(w[i], ref[i])
+                for n in spec.vecs:  # gamma, beta
+                    b.p(n).copy_(torch.rand(net.G, spec.cout) if n.endswith('.gamma') else torch.zeros(net.G, spec.cout))
 
     # nn.Module surface the reference's callers touch
     def cuda(self, device=None):
@@ -1048,6 +1067,8 @@ class Council_Trainer(nn.Module):
             for spec in net._specs():
                 by_key[spec.wname] = (net, spec, True)
                 by_key[spec.bname] = (net, spec, False)
+                for n in spec.vecs:  # a layer norm's gamma / beta: per-channel like a bias
+                    by_key[n] = (net, _VecEntry(n), False)
             out += [by_key[k] for k in net.reference_key_order() if k in by_key]
         return out
 

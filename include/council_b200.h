@@ -113,6 +113,23 @@ int cg_norm_act_bwd(const float* dz, const float* y, const float* mean, const fl
                     const float* adain, int P, int off, float* dy, float* d_adain, int G, int B,
                     int H, int W, int C, int act, int ups, void* ws, size_t ws_bytes, void* stream);
 
+/* act may also be CG_ACT_LRELU (slope 0.2, as Conv2dBlock fixes it: the discriminators' dis.norm in). */
+
+/* ---- layer norm (LayerNorm networks.py:659-686: the discriminators' dis.norm ln) ------------------------------------ */
+/* mean[G][B] and the UNBIASED std[G][B] (torch.std) of each sample over C*H*W; fp64 fixed-order fold of fp32 partials of
+ * 128 pixels, so the result is deterministic.  Needs C*H*W > 1.  Workspace: cg_ln_workspace_bytes. */
+size_t cg_ln_workspace_bytes(int G, int B, int HW, int C);
+int cg_ln_stats(const float* y, float* mean, float* std, int G, int B, int HW, int C, void* ws, size_t ws_bytes, void* stream);
+/* z = act((y - mean) / (std + eps) * gamma[g][c] + beta[g][c]); gamma, beta [G][C] (one row per member). */
+int cg_ln_act_fwd(const float* y, const float* mean, const float* std, const float* gamma, const float* beta, float eps,
+                  float* z, int G, int B, int H, int W, int C, int act, void* stream);
+/* backward of the above (the autograd of (y - mean) / (std + eps) with the unbiased std, statistics included; at std 0 the
+ * term through the std is taken as 0): dy, and dgamma / dbeta [G][C] summed over each member's samples (overwritten, like
+ * cg_conv_wgrad's db). */
+int cg_ln_act_bwd(const float* dz, const float* y, const float* mean, const float* std, const float* gamma,
+                  const float* beta, float eps, float* dy, float* dgamma, float* dbeta, int G, int B, int H, int W, int C,
+                  int act, void* ws, size_t ws_bytes, void* stream);
+
 /* backward of nn.Upsample(scale_factor=2) (networks.py:385): dx[N][H][W][C] = 2x2 fan-in sum of d_up[N][2H][2W][C] */
 int cg_upsample2x_bwd(const float* d_up, float* dx, int N, int H, int W, int C, void* stream);
 
